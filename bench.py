@@ -6,12 +6,14 @@ Workload = BASELINE.json configs[1]: one environment per GPU, 640x480 RGB-D, 100
 architecture: no checkpoint exists offline), weighted-average fusion
 (use_max_confidence=False, the policies' setting).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--batch B]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--batch B] [--dump-outputs DIR]
 
 N > 1 is launched by torchrun (one rank per GPU, env shards, NO step-path collective;
 NCCL only for the barrier and the max-over-ranks of the timing).  Prints ONE JSON line.
 `--impl reference` times the reference's own CPU algorithm (oracle port: numpy/cv2 value
-map restated from vlfm/mapping/value_map.py + fp32 HF BLIP-2 ITC) on the host cores.
+map restated from vlfm/mapping/value_map.py + fp32 HF BLIP-2 ITC) on the host cores.  `--dump-outputs DIR` writes what the last timed step
+returned (the cosine and the fused confidence / value grids) as DIR/<name>.npy: inputs are seeded, so
+two builds can be compared output for output (git ignores `bench_out/` for this).
 """
 from __future__ import annotations
 
@@ -54,16 +56,13 @@ def pin_cpu_threads() -> int:
 
 
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
-            p = json.load(fh)
-        return p, "measured"
-    except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    from vlfm_b200.utils.peaks import peaks as shared
+
+    return shared()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -134,7 +133,8 @@ def cpu_reference(steps: int, warmup: int, budget_s: float, frames, state_dict, 
         if time.perf_counter() - t_start > budget_s and len(times) >= 1:
             break
     t = float(np.mean(times))
-    return 1.0 / t, len(times), torch.get_num_threads()
+    outputs = {"cosine": np.array([c], dtype=np.float32), "confidence_map": vm._map[None], "value_map": vm._value_map[None]}
+    return 1.0 / t, len(times), torch.get_num_threads(), outputs
 
 
 def run_reference(args):
@@ -148,10 +148,12 @@ def run_reference(args):
     dims = Blip2Dims()
     sd = random_state_dict(dims, 0)
     frames = make_frames(0)
-    sps, n, threads = cpu_reference(args.steps, args.warmup, 240.0, frames, sd, dims)
+    sps, n, threads, outputs = cpu_reference(args.steps, args.warmup, 240.0, frames, sd, dims)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, outputs)
     line = {
         "impl": "reference", "metric": "value-map steps/sec (ITM+cone-fuse)", "value": sps, "unit": "env-steps/s",
-        "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 / sps, "higher_is_better": True,
+        "n_gpus": args.gpus, "steps": n, "warmup": args.warmup, "ms_per_step": 1e3 / sps, "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": WORKLOAD, "envs_per_gpu": 1,
                    "note": "CPU arm: ONE process on rank 0 with the thread count below, whatever --gpus says (not multiplied by N)"},
@@ -196,6 +198,7 @@ def run_b200(args):
         j = i % NFRAMES
         cos = itm.cosine_device(rgb[j], PROMPT)
         eng.update(cos.double().view(B, 1), depth[j], tfs[j], MIN_D, MAX_D, FOV)
+        return cos
 
     def barrier():
         if world > 1:
@@ -216,11 +219,15 @@ def run_b200(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     e0.record()
+    last_cos = None
     for i in range(K):
-        step_device(Wm + i)
+        last_cos = step_device(Wm + i)
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and K > 0:     # every rank has its own environments: rank r > 0 writes to DIR/rank<r>
+        dump_outputs(args.dump_outputs if rank == 0 else os.path.join(args.dump_outputs, f"rank{rank}"),
+                     {"cosine": last_cos, "confidence_map": eng.conf, "value_map": eng.value})
     from vlfm_b200.utils.dist import aggregate_throughput, gather_metrics, max_over_ranks
 
     ms_local = ms
@@ -239,7 +246,7 @@ def run_b200(args):
             "steps": K, "warmup": Wm, "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f16", "data": "synthetic",
             "config": {"workload": WORKLOAD if B == 1 else WORKLOAD.replace("batch=1 env/GPU", f"batch={B} env/GPU"),
-                       "envs_per_gpu": B, "l2": "per-step working set 2.0 GB of weights > 126 MB L2 (no flush needed)",
+                       "envs_per_gpu": B, "l2": "per-step working set 2.0 GB of weights > 50 MB L2 (no flush needed)",
                        "timing": "CUDA events, max over ranks"},
             "e2e": None if e2e is None else {"value": e2e, "unit": "env-steps/s", "h2d_bytes_per_step": H * W * 3 + H * W * 4 + 17 * 8,
                     "d2h_bytes_per_step": 4, "api": "BLIP2ITM.cosine + ValueMap.update_map (page-locked host numpy frames in, DMA to HBM, float out)",
@@ -319,17 +326,17 @@ def run_b200(args):
     per_rank = gather_metrics([rank, ms_local, float(eng.conf.sum().item())], dev)
     clocks = sampler.stop() if rank == 0 else None
 
-    # ---- roofline of the dominant kernel (tcgen05 GEMM): GEMM-only replay, CUDA events
+    # ---- roofline of the dominant kernel (wgmma GEMM): GEMM-only replay, CUDA events
     roof = gemm_roofline(itm.engine, B, dims)
     cpu = None
     if rank == 0 and world == 1 and not args.no_cpu:
-        sps, n, threads = cpu_reference(4, 1, 30.0, fr0, sd, dims)
+        sps, n, threads, _ = cpu_reference(4, 1, 30.0, fr0, sd, dims)
         cpu = {"value": sps, "unit": "env-steps/s", "cores": threads, "kind": "port", "host_cpus": os.cpu_count(),
                "sample": f"{n} env-steps (fp32 HF BLIP-2 ITC forward + numpy/cv2 value-map oracle), 1 warm-up"}
     if not args.no_extra and (world == 1 or args.extra_multi):
         extra = run_extras(args, dev, world, rank, local)
     elif not args.no_extra:
-        extra = {"skipped": "the extra workloads run at N=1 by default (--extra-multi runs them on every rank; profiles/r02_bench_n2.json)"}
+        extra = {"skipped": "the extra workloads run at N=1 by default (--extra-multi runs them on every rank)"}
     dog.cancel()
     emit(extra)
     if world > 1:
@@ -528,7 +535,7 @@ def gemm_roofline(engine, B, dims):
     engine._gemm, engine._gemm_x2 = orig, orig_x2
     engine.fuse_ln = orig_fuse
     torch.cuda.synchronize()
-    # dominant kernel = the fp16 tcgen05 GEMM (the ViT: 97.5 % of the FLOPs).  The Q-Former's x2 launches are a different kernel
+    # dominant kernel = the fp16 wgmma GEMM (the ViT: 97.5 % of the FLOPs).  The Q-Former's x2 launches are a different kernel
     # (three MMAs per product, float32-grade) and their residual GEMMs only split K together with the partial-sum LayerNorm launch:
     # they are counted, not replayed.
     x2_calls = [c for c in calls if c[0] is orig_x2]
@@ -550,20 +557,29 @@ def gemm_roofline(engine, B, dims):
     ms = e0.elapsed_time(e1) / reps
     ach = flops / (ms * 1e-3) / 1e12
     peak = pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
-    traffic = None
-    if B == 1:  # dram__bytes_read+write per launch from the committed ncu capture of this same workload
-        try:
-            with open(os.path.join(ROOT, "profiles", "r01_gemm_traffic_b1.json")) as fh:
-                traffic = json.load(fh)["dram_bytes_per_launch"]
-        except Exception:
-            traffic = None
-    return {"kernel": "gemm_f16_tcgen05_kernel (1-CTA 128xBN tiles at batch 1; 2-CTA persistent 256x256 tiles for large M)", "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s",
-            "frac": ach / peak, "traffic": traffic, "traffic_unit": "bytes/launch (ncu dram__bytes_read.sum+dram__bytes_write.sum, profiles/r01_gemm_traffic_b1.json)",
-            "algorithmic_bytes_per_launch": sum(2.0 * (w.numel() + a.numel()) for fn, _, a, w in calls) / len(calls), "peak_source": f"{src} (sustained dense bf16)",
+    return {"kernel": "gemm_f16_wgmma_kernel (128 x BN tiles, BN and split-K by the launch plan)", "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s",
+            "frac": ach / peak,
+            "algorithmic_bytes_per_launch": sum(2.0 * (w.numel() + a.numel()) for fn, _, a, w in calls) / len(calls), "peak_source": f"{src} (dense fp16/bf16)",
             "launches_per_step": len(calls), "flops_per_launch_avg": flops / len(calls),
-            "not_replayed": {"kernel": "gemm_f16x2_tcgen05_kernel (Q-Former, float32-grade)", "launches_per_step": len(x2_calls),
+            "not_replayed": {"kernel": "gemm_f16x2_wgmma_kernel (Q-Former, float32-grade)", "launches_per_step": len(x2_calls),
                              "share_of_gemm_flops": x2_flops / max(flops + x2_flops, 1.0)},
             "us_per_launch_avg": ms * 1e3 / len(calls), "gemm_ms_per_step": ms}
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(path, arrays):
+    """DIR/<name>.npy, float32, for every array the timed step handed back.  All of them together stay under 64 MB: an array
+    whose share would be larger is stored as a fixed sample of its flattened elements (seeded, so the same elements every run)."""
+    os.makedirs(path, exist_ok=True)
+    share = DUMP_BYTES // (4 * len(arrays)) - 64
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy() if hasattr(t, "detach") else np.asarray(t)
+        if a.size > share:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=share, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(path, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def main():
@@ -578,6 +594,10 @@ def main():
     ap.add_argument("--no-extra", action="store_true", help="skip the configs[1]@32 / [2] / [3] / [4] slices")
     ap.add_argument("--extra-batch", type=int, default=32, help="envs per GPU of the extra slices")
     ap.add_argument("--extra-multi", action="store_true", help="run the extra workloads on every rank of a multi-GPU launch too")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one returned as DIR/<name>.npy (float32): its cosine, and the confidence and value grids "
+                         "as they stand then, i.e. fused over every step the run made up to there (launch-count pass, warm-up, timed steps). Both --impl arms "
+                         "write them; rank r > 0 of a multi-GPU run writes to DIR/rank<r>")
     ap.add_argument("--extras-child", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
     if args.extras_child:

@@ -1,5 +1,5 @@
 /*
- * vlfm_b200 -- C-ABI of the B200-native VLFM perception -> value-map hot path.
+ * vlfm_b200 -- C-ABI of the VLFM perception -> value-map hot path, written for the NVIDIA H100 (sm_90a).
  *
  * The reference (bdaiinstitute/vlfm) is pure Python: the boundary it exposes is a
  * Python class surface (vlfm/mapping/*.py, vlfm/vlm/*.py).  This header is the
@@ -137,7 +137,7 @@ int vlfm_fill_small_holes(const float* d_depth, int H, int W, double area_thresh
                           int32_t* d_status, void* stream);
 
 /* ---------------------------------------------------------------- dense (VLM) ---- */
-/* fp16 x fp16 -> fp32-accumulate GEMM on tcgen05 tensor cores, TMA-fed:
+/* fp16 x fp16 -> fp32-accumulate GEMM on Hopper tensor cores (wgmma), TMA-fed:
  *   out[M,N] = epilogue(A[M,K] @ W[N,K]^T + bias[N])
  * A, W row-major fp16 (K contiguous, K % 8 == 0).
  * epilogue: 0 = bias -> fp16 out; 1 = bias + GELU(erf) -> fp16 out;
@@ -189,7 +189,7 @@ int vlfm_attention_f16(const void* d_q, const void* d_k, const void* d_v, void* 
 /* ---- "x2" path: float32-grade Q-Former on the fp16 tensor path.  The reference runs the Q-Former in float32 (lavis casts
  * only the ViT to half); fp16 operands there alone move the ITC cosine by ~3e-5 (measured on the fp32 oracle), the ViT's by 1e-6.
  * An x2 operand is a pair of fp16 arrays (hi, lo) with value = hi + lo / 2048, hi = fp16(v), lo = fp16((v - hi) * 2048).
- * vlfm_gemm_f16x2: out = epilogue(A @ W^T + bias), A and W x2 operands, three tcgen05.mma per K step into two TMEM
+ * vlfm_gemm_f16x2: out = epilogue(A @ W^T + bias), A and W x2 operands, three wgmma per K step into two register
  *   accumulators (hi.hi | lo.hi + hi.lo).  epilogue: VLFM_EPI_BIAS_F32, VLFM_EPI_BIAS_RESID_F32, VLFM_EPI_BIAS_GELU_F16X2 (GELU, output
  *   written as x2 operands d_out / d_out_lo).
  * vlfm_gemm_f16x2_resid_ln: x += ...; LayerNorm(x) -> x2 operands (+ fp32), deterministic split-K like vlfm_gemm_f16_resid_ln.

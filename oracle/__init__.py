@@ -14,12 +14,12 @@ Contents
                         ``vlfm/utils/img_utils.py`` / ``geometry_utils.py`` it calls).
 ``obstacle_map_oracle`` restatement of ``vlfm/mapping/obstacle_map.py`` including the
                         third-party ``frontier_exploration`` functions it calls
-                        (that package is absent from /root/reference: parity for the
+                        (that package is absent from $VLFM_REFERENCE: parity for the
                         fog-of-war / frontier half is UNPINNED, see DESIGN.md).
 ``blip2_oracle``        architecture-equivalent fp32 BLIP-2 ITC forward built on
                         HF transformers (LAVIS is absent: parity UNPINNED w.r.t. LAVIS).
-``ref_import``          imports the real reference from /root/reference (container only;
-                        used to pin the restatements and to generate tests/golden/*).
+``ref_import``          imports the real reference from a checkout named by $VLFM_REFERENCE
+                        (used only to generate tests/golden/*).
 
 Pinning status is recorded per module in its header and in DESIGN.md.
 """

@@ -3,7 +3,7 @@ two third-party functions it calls.
 
 TEST INFRASTRUCTURE.  PARITY UNPINNED.  ``frontier_exploration`` is an unpinned git
 dependency (pyproject.toml:25: git+https://github.com/naokiyokoyama/frontier_exploration.git)
-that is NOT in /root/reference and cannot be fetched here; the reference has no test or
+that is NOT in $VLFM_REFERENCE and cannot be fetched here; the reference has no test or
 golden vector at this boundary.  ``reveal_fog_of_war`` and ``detect_frontier_waypoints``
 below restate that package's published algorithm from its call sites
 (obstacle_map.py:117-124, :164-168) and from the rules recorded in SURVEY.md section 8c;

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE.  PARITY UNPINNED: the package
 (git+https://github.com/naokiyokoyama/frontier_exploration.git, no commit pinned,
-/root/reference/pyproject.toml:25) is NOT present in /root/reference and cannot be
+$VLFM_REFERENCE/pyproject.toml:25) is NOT present in $VLFM_REFERENCE and cannot be
 fetched; no reference test pins its results.  The functions are filled in by
 oracle/explore_oracle.py (see there for the rule-by-rule restatement).
 """

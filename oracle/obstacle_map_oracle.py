@@ -5,7 +5,7 @@ Obstacle half (:86-109, hole fill -> point cloud -> height band -> np.rint scatt
 k x k dilation): PINNED bit-for-bit against the real reference class (imported with
 ``frontier_exploration`` stubbed, tests/test_oracle_obstacle.py + golden fixtures).
 Explore half (:114-169): built on oracle/frontier_exploration_oracle.py, whose source
-package is absent from /root/reference -> parity UNPINNED for that half.
+package is absent from $VLFM_REFERENCE -> parity UNPINNED for that half.
 """
 from __future__ import annotations
 

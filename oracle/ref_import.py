@@ -1,7 +1,7 @@
-"""Import the REAL reference classes from /root/reference (build container only).
+"""Import the REAL reference classes from a checkout of bdaiinstitute/vlfm named by $VLFM_REFERENCE.
 
-TEST INFRASTRUCTURE.  /root/reference does not exist on the GPU box: nothing that runs
-there may call this module (tests that use it are skipped when the tree is absent).
+FIXTURE GENERATION ONLY (oracle/make_golden.py).  No test and nothing on the product path calls this module: the tests
+compare against what the reference computed, stored under tests/golden/.
 
 ``vlfm.mapping.value_map`` imports cleanly (cv2 + numpy only).
 ``vlfm.mapping.obstacle_map`` needs ``frontier_exploration`` (third-party, unpinned
@@ -15,11 +15,11 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = "/root/reference"
+REFERENCE_ROOT = os.environ.get("VLFM_REFERENCE", "")
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "vlfm", "mapping"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "vlfm", "mapping"))
 
 
 def _ensure_path() -> None:
@@ -62,6 +62,33 @@ def geometry_utils():
     import vlfm.utils.geometry_utils as g  # type: ignore
 
     return g
+
+
+def base_map_class():
+    _ensure_path()
+    from vlfm.mapping.base_map import BaseMap  # type: ignore
+
+    return BaseMap
+
+
+def frontier_map_class(encoder_cls):
+    """vlfm.mapping.frontier_map with its HTTP encoder client replaced by ``encoder_cls``."""
+    _ensure_path()
+    stub = types.ModuleType("vlfm.vlm.blip2itm")
+    stub.BLIP2ITMClient = encoder_cls
+    saved = {k: sys.modules.get(k) for k in ("vlfm.vlm.blip2itm", "vlfm.mapping.frontier_map")}
+    sys.modules["vlfm.vlm.blip2itm"] = stub
+    sys.modules.pop("vlfm.mapping.frontier_map", None)
+    try:
+        from vlfm.mapping.frontier_map import FrontierMap  # type: ignore
+
+        return FrontierMap
+    finally:
+        for k, v in saved.items():
+            if v is None:
+                sys.modules.pop(k, None)
+            else:
+                sys.modules[k] = v
 
 
 def img_utils():

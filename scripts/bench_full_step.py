@@ -1,4 +1,4 @@
-"""BASELINE.json configs[2]: the FULL policy step for a batch of environments on one B200 (vlfm_b200/utils/full_step.py:
+"""BASELINE.json configs[2]: the FULL policy step for a batch of environments on one H100 (vlfm_b200/utils/full_step.py:
 GroundingDINO detect + BLIP-2 ITC + batched ObstacleMap update + ValueMap fuse + frontier scoring) with per-component
 CUDA-event times.  bench.py runs the same harness for its `extra` block; this script is for one-off sweeps.
 
@@ -13,6 +13,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from vlfm_b200.utils.full_step import FullStep  # noqa: E402
+from vlfm_b200.utils.peaks import peaks  # noqa: E402
 from vlfm_b200.vlm.blip2_config import Blip2Dims, random_state_dict  # noqa: E402
 from vlfm_b200.vlm.blip2itm import BLIP2ITM  # noqa: E402
 
@@ -39,8 +40,10 @@ def main():
     fs = FullStep(dev, a.batch, a.hw[0], a.hw[1], a.grid, a.ppm, itm, gd, frames_per_env=a.steps + a.warmup, hole_thresh=a.hole_thresh,
                   bound_m=0.015 * a.grid)
     r = fs.run(a.steps, a.warmup)
-    r["grid_rooflines"] = fs.grid_rooflines(6564.8)
-    r["config"] = {"workload": f"full step, batch={a.batch} envs, {a.hw[1]}x{a.hw[0]} RGB-D, {a.grid}^2 grid at {a.ppm} px/m, 1xB200", "data": "synthetic"}
+    pk, src = peaks()
+    r["grid_rooflines"] = fs.grid_rooflines(float(pk["hbm_gbs"]))
+    r["peak_hbm_gbs"], r["peak_source"] = float(pk["hbm_gbs"]), src
+    r["config"] = {"workload": f"full step, batch={a.batch} envs, {a.hw[1]}x{a.hw[0]} RGB-D, {a.grid}^2 grid at {a.ppm} px/m, 1xH100", "data": "synthetic"}
     print(json.dumps(r))
 
 

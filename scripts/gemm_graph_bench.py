@@ -1,4 +1,3 @@
-# NOTE: needs a development build of the library (NVCC flag -DVLFM_DEV_PROBES): the probe entry points are not in the shipped C-ABI.
 """Per-shape GEMM timing at full clocks: 200 back-to-back launches captured in a CUDA graph
 (no CPU launch bound), optional sweep of the tile plan via VLFM_GEMM_FORCE=bn:splits."""
 import os, sys, itertools
@@ -41,26 +40,4 @@ for (M, Nn, K, epi) in SHAPES:
             for sp in ((1, 2, 3, 4, 6, 8) if epi == 2 else (1,)):
                 os.environ["VLFM_GEMM_FORCE"] = f"{bn}:{sp}"
                 line += f" | {bn}:{sp}={bench(M, Nn, K, epi):.2f}"
-                if len(sys.argv) > 2 and sp <= 4:
-                    os.environ["VLFM_GEMM_FORCE"] = f"{bn}:{sp}:1"
-                    line += f" {bn}:{sp}:sh={bench(M, Nn, K, epi):.2f}"
     print(line, flush=True)
-
-if len(sys.argv) > 1 and sys.argv[1] == "timeline":
-    # phases of CTA (0,0,0) of the LAST launch of a 200-launch graph (sustained clocks)
-    import numpy as np
-    from vlfm_b200 import _lib
-    lib = _lib.load()
-    buf = torch.zeros(8 + 4096, dtype=torch.int64, device="cuda")
-    names = ["start", "setup", "depwait", "stage0(w1)", "lastmma(w1)", "accready(w2)", "epidone"]
-    for (M, Nn, K, epi) in SHAPES[:4]:
-        os.environ.pop("VLFM_GEMM_FORCE", None)
-        lib.vlfm_gemm_debug_timeline(buf.data_ptr())
-        t_us = bench(M, Nn, K, epi)
-        lib.vlfm_gemm_debug_timeline(None)
-        t = buf.cpu().tolist()
-        st = np.array(t[8:8 + 4096:2]); en = np.array(t[9:9 + 4096:2]); ok = st > 0
-        rel = [(t[i] - t[0]) / 1.965e3 for i in range(7)]
-        print(f"{M}x{Nn}x{K} epi{epi}: {t_us:.2f} us/launch | " + " ".join(f"{n}={v:.2f}" for n, v in zip(names, rel)) +
-              f" | ctas={ok.sum()} skew={(st[ok].max()-st[ok].min())/1e3:.2f} life_avg={(en[ok]-st[ok]).mean()/1e3:.2f} life_max={(en[ok]-st[ok]).max()/1e3:.2f} span={(en[ok].max()-st[ok].min())/1e3:.2f}")
-        buf.zero_()

@@ -15,7 +15,7 @@ def timeit(fn, it=5):
     e1.record(); torch.cuda.synchronize()
     return e0.elapsed_time(e1) / it
 print("PDL", os.environ.get("VLFM_PDL", "1"), "(each kernel: 10us pre-wait + 10us post-wait; 20us = no overlap, 10us = full overlap)")
-for blocks, smem in [(148, 0), (148, 100 * 1024), (148, 200 * 1024), (100, 200 * 1024)]:
+for blocks, smem in [(132, 0), (132, 100 * 1024), (132, 200 * 1024), (100, 200 * 1024)]:
     t_s = timeit(lambda: run(50, blocks, smem)) * 1e3 / 50
     s = torch.cuda.Stream()
     with torch.cuda.stream(s):

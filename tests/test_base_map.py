@@ -1,10 +1,8 @@
-"""BaseMap conversions (vlfm/mapping/base_map.py:35-60): explicit formulae everywhere, the live reference class where present."""
-import sys
-
+"""BaseMap conversions (vlfm/mapping/base_map.py:35-60): explicit formulae, and what the reference class returned (stored fixtures)."""
 import numpy as np
 import pytest
 
-from conftest import has_reference
+from oracle.live_cases import base_map_points
 from vlfm_b200.mapping.base_map import BaseMap
 
 
@@ -40,16 +38,10 @@ def test_conversions_match_reference_arithmetic(size, ppm):
     assert m._camera_positions == []
 
 
-@pytest.mark.skipif(not has_reference(), reason="/root/reference not present")
-def test_conversions_match_live_reference_class():
-    if "/root/reference" not in sys.path:
-        sys.path.insert(0, "/root/reference")
-    from vlfm.mapping.base_map import BaseMap as RefBaseMap  # type: ignore
-
-    rng = np.random.default_rng(5)
-    ref, got = RefBaseMap(size=1000), BaseMap(size=1000)
-    pts = rng.uniform(-20, 20, (1000, 2))
-    assert np.array_equal(got._xy_to_px(pts), ref._xy_to_px(pts))
-    cells = rng.uniform(0, 1000, (300, 2))
-    assert np.array_equal(got._px_to_xy(cells), ref._px_to_xy(cells))
-    assert np.array_equal(got._episode_pixel_origin, ref._episode_pixel_origin) and got.pixels_per_meter == ref.pixels_per_meter
+def test_conversions_match_live_reference_class(live_golden):
+    ref, got = live_golden("base_map"), BaseMap(size=1000)
+    pts, cells = base_map_points()
+    px = got._xy_to_px(pts)
+    assert px.dtype.kind == ref["px"].dtype.kind and np.array_equal(px, ref["px"])
+    assert np.array_equal(got._px_to_xy(cells), ref["xy"])
+    assert np.array_equal(got._episode_pixel_origin, ref["origin"]) and got.pixels_per_meter == ref["ppm"]

@@ -1,34 +1,11 @@
 """FrontierMap (vlfm/mapping/frontier_map.py:10-77): host bookkeeping around one cosine call per update that introduces a
-new frontier.  Checked against explicit expectations everywhere, and against the REAL reference class (its HTTP encoder
-replaced by the same scripted one) where /root/reference exists."""
-import sys
-import types
-
+new frontier.  Checked against explicit expectations, and against what the REAL reference class (its HTTP encoder replaced by
+the same scripted one) did on the same streams (stored fixtures)."""
 import numpy as np
 import pytest
 
-from conftest import has_reference
+from oracle.live_cases import FRONTIER_SEEDS, ScriptedEncoder, frontier_stream
 from vlfm_b200.mapping.frontier_map import FrontierMap
-
-
-class ScriptedEncoder:
-    def __init__(self):
-        self.calls = 0
-
-    def cosine(self, image, text):
-        self.calls += 1
-        return 0.1 * self.calls + float(image.sum() % 7) * 1e-3
-
-
-def _stream(seed, steps=30):
-    rng = np.random.default_rng(seed)
-    pool = [rng.uniform(-5, 5, 2).round(2) for _ in range(12)]
-    out = []
-    for _ in range(steps):
-        k = int(rng.integers(0, 6))
-        idx = rng.choice(len(pool), size=k, replace=False)
-        out.append(([pool[i].copy() for i in idx], rng.integers(0, 255, (4, 4, 3), dtype=np.uint8)))
-    return out
 
 
 def test_update_sort_reset_semantics():
@@ -51,34 +28,17 @@ def test_update_sort_reset_semantics():
     assert enc.calls == 2 and fm.frontiers == []
 
 
-@pytest.mark.skipif(not has_reference(), reason="/root/reference not present")
-@pytest.mark.parametrize("seed", [0, 1, 2])
-def test_matches_live_reference(seed):
-    stub = types.ModuleType("vlfm.vlm.blip2itm")
-    stub.BLIP2ITMClient = ScriptedEncoder
-    saved = {k: sys.modules.get(k) for k in ("vlfm.vlm.blip2itm", "vlfm.mapping.frontier_map")}
-    sys.modules["vlfm.vlm.blip2itm"] = stub
-    sys.modules.pop("vlfm.mapping.frontier_map", None)
-    if "/root/reference" not in sys.path:
-        sys.path.insert(0, "/root/reference")
-    try:
-        from vlfm.mapping.frontier_map import FrontierMap as RefFrontierMap  # type: ignore
-
-        ref, got = RefFrontierMap(), FrontierMap(encoder=ScriptedEncoder())
-        ref.frontiers = []
-        for locs, img in _stream(seed):
-            ref.update(locs, img, "a chair")
-            got.update(locs, img, "a chair")
-            assert len(ref.frontiers) == len(got.frontiers)
-            for r, g in zip(ref.frontiers, got.frontiers):
-                assert np.array_equal(r.xyz, g.xyz) and r.cosine == g.cosine
-            if ref.frontiers:
-                (rp, rv), (gp, gv) = ref.sort_waypoints(), got.sort_waypoints()
-                assert rv == gv and np.array_equal(rp, gp)
-        assert ref.encoder.calls == got.encoder.calls
-    finally:
-        for k, v in saved.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
+@pytest.mark.parametrize("seed", FRONTIER_SEEDS)
+def test_matches_live_reference(seed, live_golden):
+    ref, got = live_golden("frontier_map"), FrontierMap(encoder=ScriptedEncoder())
+    for k, (locs, img) in enumerate(frontier_stream(seed)):
+        got.update(locs, img, "a chair")
+        key = f"s{seed}_t{k}_"
+        r_xyz, r_cos = ref[key + "xyz"], ref[key + "cos"]
+        assert len(r_cos) == len(got.frontiers)
+        for x, c, g in zip(r_xyz, r_cos, got.frontiers):
+            assert np.array_equal(x, g.xyz) and c == g.cosine
+        if got.frontiers:
+            gp, gv = got.sort_waypoints()
+            assert list(ref[key + "sorted_vals"]) == gv and np.array_equal(ref[key + "sorted_pts"], gp)
+    assert int(ref[f"s{seed}_calls"]) == got.encoder.calls and got.encoder.calls > 3

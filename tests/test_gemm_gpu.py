@@ -1,4 +1,4 @@
-"""tcgen05 GEMM vs a plain PyTorch fp32 reference of the same op (fp16 inputs, fp32
+"""wgmma GEMM vs a plain PyTorch fp32 reference of the same op (fp16 inputs, fp32
 accumulation): tolerance 2e-3 relative to the output scale."""
 import numpy as np
 import pytest

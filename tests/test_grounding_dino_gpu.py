@@ -105,7 +105,7 @@ def test_tc_linear_and_cast_vs_torch():
 
 def test_accelerated_primitives_are_installed(pair):
     _, g = pair
-    # 6 encoder deformable layers rewritten whole, 6 decoder cross-attentions, every other nn.Linear on the tcgen05 GEMM
+    # 6 encoder deformable layers rewritten whole, 6 decoder cross-attentions, every other nn.Linear on the wgmma GEMM
     assert g.accel["deformable_layers"] == 6 and g.accel["decoder_layers"] == 6 and g.accel["fusion_layers"] == 6, g.accel
     assert g.accel["linear"] > 60, g.accel
 
@@ -277,7 +277,7 @@ def test_batch1_cuda_graph_replay_matches_eager(pair):
     r = [t.clone() for t in g.raw_outputs(img1, ids)]                 # replay
     ee, ge = metrics(e0[0], e0[1], e1[0], e1[1]), metrics(e0[0], e0[1], r[0], r[1])
     print("eager vs eager (confidence, box-set):", ee, " graph vs eager:", ge)
-    # run-to-run level observed on B200: 3e-4 .. 1.3e-3 mean confidence difference (a broken replay is off by > 1e-1)
+    # run-to-run differences are a few 1e-4 .. 1e-3 of mean confidence (a broken replay is off by > 1e-1)
     assert ge[0] <= max(5e-3, 3 * ee[0]) and ge[1] <= max(1e-3, 3 * ee[1])
     torch.cuda.synchronize(); t0 = time.perf_counter()
     for _ in range(10):

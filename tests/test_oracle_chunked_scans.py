@@ -3,7 +3,7 @@
 * `ppt_distance_warp` (csrc/explore.cu) evaluates cv2.pointPolygonTest in 32 contiguous chunks and combines the chunk results in
   order with the sequential "first strictly smaller" comparison -- here the same chunked scan in numpy against the oracle's
   sequential one;
-* the x2 operand arithmetic of `gemm_f16x2_tcgen05_kernel` (csrc/gemm_tcgen05.cu): v = hi + lo/2048 with fp16 pairs and the
+* the x2 operand arithmetic of `gemm_f16x2_wgmma_kernel` (csrc/gemm_wgmma.cu): v = hi + lo/2048 with fp16 pairs and the
   three-product expansion hi.hi + (lo.hi + hi.lo)/2048 -- here in numpy against float64."""
 import numpy as np
 

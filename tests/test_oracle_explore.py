@@ -1,10 +1,11 @@
 """Explore half of the obstacle map: the cv2-based restatement and the cv2-free one agree, and the reference's
-own ObstacleMap code (run with the restated frontier_exploration functions injected) agrees with both."""
+own ObstacleMap code (run with the restated frontier_exploration functions injected; its outputs are stored fixtures) agrees
+with both."""
 import numpy as np
 import pytest
 
 import oracle.explore_oracle as ex
-from conftest import has_reference
+from oracle.live_cases import explore_frames
 from oracle.obstacle_map_oracle import ObstacleMapOracle
 from vlfm_b200.utils.synthetic import focal_from_hfov, trajectory
 
@@ -43,17 +44,14 @@ def test_backends_agree_at_the_map_border():
             assert np.array_equal(ea, eb) and fa.shape == fb.shape and np.array_equal(fa, fb) and np.array_equal(xa, xb)
 
 
-@pytest.mark.skipif(not has_reference(), reason="/root/reference not present")
-def test_reference_class_with_injected_functions():
-    from oracle import ref_import
-
-    RO = ref_import.obstacle_map_class()
-    r = RO(0.61, 0.88, 0.18, area_thresh=1.5, hole_area_thresh=-1, size=400)
+def test_reference_class_with_injected_functions(live_golden):
+    ref = live_golden("explore")
     o = ObstacleMapOracle(0.61, 0.88, 0.18, area_thresh=1.5, hole_area_thresh=-1, size=400)
     fx = focal_from_hfov(160)
-    for f in trajectory(7, 6, h=120, w=160, bound_m=4):
-        r.update_map(f.depth, f.tf, 0.5, 5.0, fx, fx, np.deg2rad(79))
+    for k, f in enumerate(explore_frames()):
         o.update_map(f.depth, f.tf, 0.5, 5.0, fx, fx, np.deg2rad(79))
-        assert np.array_equal(r.explored_area, o.explored_area)
-        assert np.array_equal(np.asarray(r._frontiers_px), np.asarray(o._frontiers_px))
-        assert np.array_equal(np.asarray(r.frontiers), np.asarray(o.frontiers))
+        explored = np.unpackbits(ref[f"explored{k}"])[: 400 * 400].reshape(400, 400)
+        assert explored.any()
+        assert np.array_equal(explored.astype(bool), np.asarray(o.explored_area, dtype=bool))
+        assert np.array_equal(ref[f"frontiers_px{k}"], np.asarray(o._frontiers_px))
+        assert np.array_equal(ref[f"frontiers{k}"], np.asarray(o.frontiers))

@@ -1,12 +1,12 @@
 """oracle/object_map_oracle.py: DBSCAN restatement vs scikit-learn's implementation; the whole class vs the REAL reference
-class (vlfm/mapping/object_point_cloud_map.py) imported with a stub open3d."""
+class (vlfm/mapping/object_point_cloud_map.py, run with a stub open3d; its outputs are stored fixtures)."""
 import cv2
 import numpy as np
 import pytest
 
-from conftest import has_reference
 from oracle import object_map_oracle as om
-from vlfm_b200.utils.synthetic import focal_from_hfov, make_object_mask, trajectory
+from oracle.live_cases import fingerprint, object_scenario
+from vlfm_b200.utils.synthetic import make_object_mask
 
 
 def _clustered(rng, n):
@@ -41,38 +41,32 @@ def test_erode_restatement():
         assert np.array_equal(cv2.erode(m * 255, None, iterations=k), om.erode_mask_numpy(m, k))
 
 
-def _scenario(seed, steps=6, h=240, w=320):
-    rng = np.random.default_rng(100 + seed)
-    fx = focal_from_hfov(w)
-    out = []
-    for i, f in enumerate(trajectory(seed, steps, h=h, w=w, bound_m=6.0)):
-        side = ["any", "left", "any", "right", "any"][i % 5]
-        mask = make_object_mask(rng, h, w, side)
-        depth = f.depth.copy()
-        if i % 3 == 2:
-            depth[mask > 0] = np.float32(0.98)                                # a far detection: out-of-range ids
-        out.append((depth, mask, f.tf, fx))
-    return out
+def _same(ref, key, a):
+    """`a` against the fingerprint oracle/make_golden.py stored of the reference's array: shape, dtype and the SHA-256 of the
+    bytes, i.e. equality of the whole array (clouds of 10^4..10^5 points are too large to store)."""
+    got = fingerprint(np.asarray(a))
+    assert np.array_equal(got["shape"], ref[key + "_shape"]) and str(got["dtype"]) == str(ref[key + "_dtype"]), key
+    assert np.array_equal(got["rows"], ref[key + "_rows"]), key
+    return str(got["sha256"]) == str(ref[key + "_sha256"])
 
 
-@pytest.mark.skipif(not has_reference(), reason="/root/reference not present")
 @pytest.mark.parametrize("use_dbscan", [True, False])
-def test_oracle_class_matches_the_reference_class(use_dbscan):
-    from oracle import ref_import
-
-    R = ref_import.object_map_module().ObjectPointCloudMap
+def test_oracle_class_matches_the_reference_class(use_dbscan, live_golden):
+    ref = live_golden("object_map")
+    seen = 0
     for seed in range(3):
-        r, o = R(erosion_size=2), om.ObjectPointCloudMapOracle(erosion_size=2)
-        r.reset()
-        r.use_dbscan = o.use_dbscan = use_dbscan
-        for depth, mask, tf, fx in _scenario(seed):
-            for m in (r, o):
-                np.random.seed(7 + seed)
-                m.update_map("chair", depth, mask, tf, 0.5, 5.0, fx, fx)
-                m.update_explored(tf, 5.0, np.deg2rad(79))
-            assert r.has_object("chair") == o.has_object("chair")
-            if r.has_object("chair"):
-                assert np.array_equal(r.clouds["chair"], o.clouds["chair"])
+        o = om.ObjectPointCloudMapOracle(erosion_size=2)
+        o.use_dbscan = use_dbscan
+        for k, (depth, mask, tf, fx) in enumerate(object_scenario(seed)):
+            np.random.seed(7 + seed)
+            o.update_map("chair", depth, mask, tf, 0.5, 5.0, fx, fx)
+            o.update_explored(tf, 5.0, np.deg2rad(79))
+            key = f"d{int(use_dbscan)}_s{seed}_t{k}_"
+            assert bool(ref[key + "has"]) == o.has_object("chair")
+            if o.has_object("chair"):
+                seen += 1
+                assert _same(ref, key + "cloud", o.clouds["chair"])
                 pos = tf[:2, 3] + 0.3
-                assert np.array_equal(r.get_best_object("chair", pos), o.get_best_object("chair", pos))
-                assert np.array_equal(r.get_target_cloud("chair"), o.get_target_cloud("chair"))
+                assert np.array_equal(ref[key + "best"], o.get_best_object("chair", pos))
+                assert _same(ref, key + "target", o.get_target_cloud("chair"))
+    assert seen >= 6

@@ -1,25 +1,23 @@
 import numpy as np
 import pytest
 
-from conftest import has_reference
+from oracle.live_cases import OBSTACLE_CASES, OBSTACLE_HOLES
 from oracle.obstacle_map_oracle import ObstacleMapOracle
 from vlfm_b200.utils.synthetic import focal_from_hfov, trajectory
 
 
-@pytest.mark.skipif(not has_reference(), reason="/root/reference not present")
-@pytest.mark.parametrize("hole", [-1, 100000])
-def test_obstacle_half_matches_live_reference(hole):
-    from oracle import ref_import
-
-    RO = ref_import.obstacle_map_class()
-    for seed, (h, w), size, ppm in [(0, (240, 320), 600, 20), (2, (240, 320), 1500, 50)]:
-        r = RO(0.61, 0.88, 0.18, area_thresh=1.5, hole_area_thresh=hole, size=size, pixels_per_meter=ppm)
+@pytest.mark.parametrize("hole", OBSTACLE_HOLES)
+def test_obstacle_half_matches_live_reference(hole, live_golden):
+    ref = live_golden("obstacle")
+    for i, (seed, (h, w), size, ppm) in enumerate(OBSTACLE_CASES):
         o = ObstacleMapOracle(0.61, 0.88, 0.18, area_thresh=1.5, hole_area_thresh=hole, size=size, pixels_per_meter=ppm)
         fx = focal_from_hfov(w)
         for f in trajectory(seed, 4, h=h, w=w, bound_m=5):
-            r.update_map(f.depth, f.tf, 0.5, 5.0, fx, fx, np.deg2rad(79), explore=False)
             o.update_map(f.depth, f.tf, 0.5, 5.0, fx, fx, np.deg2rad(79), explore=False)
-        assert np.array_equal(r._map, o._map) and np.array_equal(r._navigable_map, o._navigable_map)
+        r_map = np.unpackbits(ref[f"h{hole}_map{i}"])[: size * size].reshape(size, size).astype(bool)
+        r_nav = np.unpackbits(ref[f"h{hole}_nav{i}"])[: size * size].reshape(size, size).astype(bool)
+        assert r_map.any() and not r_nav.all()
+        assert np.array_equal(r_map, o._map) and np.array_equal(r_nav, o._navigable_map)
 
 
 def _depth_with_holes(seed, h=60, w=80):

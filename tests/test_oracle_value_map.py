@@ -1,5 +1,5 @@
 """Pin oracle/value_map_oracle.py: (1) against the committed fixtures generated from the
-real reference, (2) against the live reference when /root/reference exists,
+real reference, (2) against what the reference class computed on two more scenarios (stored fixtures),
 (3) cv2 and numpy primitive back-ends agree bit for bit."""
 import glob
 import hashlib
@@ -8,7 +8,7 @@ import os
 import numpy as np
 import pytest
 
-from conftest import has_reference
+from oracle.live_cases import VALUE_CASES
 from oracle.value_map_oracle import ValueMapOracle
 from vlfm_b200.utils.synthetic import trajectory
 
@@ -56,38 +56,25 @@ def test_oracle_matches_golden(golden_dir, prims):
         assert np.array_equal(sw, z["sorted_wp"]) and np.allclose(np.asarray(sv, float), z["sorted_val"], rtol=0, atol=0)
 
 
-@pytest.mark.skipif(not has_reference(), reason="/root/reference not present")
-def test_oracle_matches_live_reference():
-    from oracle import ref_import
-
-    RV = ref_import.value_map_class()
-    for ch, maxc, fus, size, seed in [(1, False, "default", 700, 21), (2, True, "default", 500, 22)]:
-        RV._confidence_masks.clear()
-        r = RV(ch, size=size, use_max_confidence=maxc, fusion_type=fus)
+def test_oracle_matches_live_reference(live_golden):
+    ref = live_golden("value_map")
+    for i, (ch, maxc, fus, size, seed) in enumerate(VALUE_CASES):
         o = ValueMapOracle(ch, size=size, use_max_confidence=maxc, fusion_type=fus, prims="numpy")
         rng = np.random.default_rng(seed)
         for f in trajectory(seed, 5, bound_m=size / 40 - 6):
-            v = rng.random(ch)
-            r.update_map(v, f.depth, f.tf, 0.5, 5.0, FOV)
-            o.update_map(v, f.depth, f.tf, 0.5, 5.0, FOV)
-        assert np.array_equal(r._map, o._map) and np.array_equal(r._value_map, o._value_map)
+            o.update_map(rng.random(ch), f.depth, f.tf, 0.5, 5.0, FOV)
+        r_map, r_value = ref[f"map{i}"], ref[f"value{i}"]
+        assert r_map.any() and r_map.dtype == o._map.dtype and r_value.dtype == o._value_map.dtype
+        assert np.array_equal(r_map, o._map) and np.array_equal(r_value, o._value_map)
 
 
-@pytest.mark.skipif(not has_reference(), reason="/root/reference not present")
-def test_oracle_ppm40_matches_patched_reference():
+def test_oracle_ppm40_matches_patched_reference(live_golden):
     """configs[4]/[5] geometry: the reference needs `pixels_per_meter` patched and its cone cache cleared
     (value_map.py:65, :339); the oracle takes ppm as a parameter."""
-    from oracle import ref_import
-
-    RV = ref_import.value_map_class()
-    RV._confidence_masks.clear()
-    r = RV(1, size=1000, use_max_confidence=False)
-    r.pixels_per_meter = 40
+    ref = live_golden("value_map")
     o = ValueMapOracle(1, size=1000, use_max_confidence=False, pixels_per_meter=40, prims="numpy")
     rng = np.random.default_rng(9)
     for f in trajectory(62, 2, h=128, w=128, bound_m=6.0):
-        v = rng.random(1)
-        r.update_map(v, f.depth, f.tf, 0.5, 5.0, FOV)
-        o.update_map(v, f.depth, f.tf, 0.5, 5.0, FOV)
-    RV._confidence_masks.clear()
-    assert np.array_equal(r._map, o._map) and np.array_equal(r._value_map, o._value_map)
+        o.update_map(rng.random(1), f.depth, f.tf, 0.5, 5.0, FOV)
+    assert ref["ppm40_map"].any()
+    assert np.array_equal(ref["ppm40_map"], o._map) and np.array_equal(ref["ppm40_value"], o._value_map)

@@ -1,4 +1,4 @@
-"""The float32-grade "x2" path of the Q-Former (fp16 pairs hi + lo/2048 on the tcgen05 GEMM, float32 attention) against
+"""The float32-grade "x2" path of the Q-Former (fp16 pairs hi + lo/2048 on the wgmma GEMM, float32 attention) against
 float64 references of the same ops.  Tolerances are float32-arithmetic sized (1e-6 of the output scale), three orders of magnitude
 below the plain fp16-operand GEMM's 2e-3."""
 import ctypes

@@ -1,4 +1,4 @@
-"""Build libvlfm_b200.so in-tree with nvcc for sm_100a (no JIT cache, no CPU fallback)."""
+"""Build libvlfm_b200.so in-tree with nvcc for sm_90a (no JIT cache, no CPU fallback)."""
 from __future__ import annotations
 
 import os
@@ -10,8 +10,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvlfm_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100: wgmma and TMA need the arch-specific target
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    *ARCH, "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -50,7 +51,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=min(8, max(1, len(jobs)))) as ex:
         list(ex.map(run, jobs))
     if jobs or force or _stale(LIB, objs):
-        run([NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB, *objs, "-cudart", "static"])
+        run([NVCC, *ARCH, "-shared", "-o", LIB, *objs, "-cudart", "static"])
     return LIB
 
 

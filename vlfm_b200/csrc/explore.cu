@@ -1,4 +1,4 @@
-// Explore half of the obstacle map on the GPU (sm_100a): fog-of-war, explored-area component selection,
+// Explore half of the obstacle map on the GPU (sm_90a): fog-of-war, explored-area component selection,
 // frontier waypoints -- for a BATCH of environments per call.
 //
 // Reference: vlfm/mapping/obstacle_map.py:114-169 and the two `frontier_exploration` functions it calls
@@ -1257,11 +1257,11 @@ size_t carve(ExEnv* e, uint8_t* base, size_t frame_cells, int frame_side, int ma
   return o;
 }
 
-inline int nblk(long n, int t = 256, int cap = 2368) { long b = (n + t - 1) / t; return (int)(b < 1 ? 1 : (b > cap ? cap : b)); }
+inline int nblk(long n, int t = 256, int cap = 2112) { long b = (n + t - 1) / t; return (int)(b < 1 ? 1 : (b > cap ? cap : b)); }
 // Launch geometry of the batched sequences is FIXED (every kernel is grid-stride over its frame): the sequence of a call depends
 // on the batch size only, so a caller can capture it in a CUDA graph and replay it with new per-environment records.
-inline int gx_cells(int B) { return B >= 16 ? 148 : (B >= 4 ? 296 : 592); }     // blocks.x of the per-cell kernels
-constexpr int GX_ROWS = 74;                                                     // blocks.x of the per-row kernels (8 warps each)
+inline int gx_cells(int B) { return B >= 16 ? 132 : (B >= 4 ? 264 : 528); }     // blocks.x of the per-cell kernels
+constexpr int GX_ROWS = 66;                                                     // blocks.x of the per-row kernels (8 warps each)
 
 // external contours of image `id` of every environment: CCL fg/bg, top-level roots in cv2 order, traced chains.
 // n_max / h_max / per_max: the largest image over the environments of the call.
@@ -1492,7 +1492,7 @@ extern "C" int vlfm_fill_small_holes_batch(const float* d_depth, int H, int W, i
     rc = check_cuda(cudaFuncSetAttribute(fill_small_contours_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_words * 4), "attr(fill_small_contours)");
     if (rc) return rc; cfg = true;
   }
-  const int fb = B >= 8 ? 37 : (B >= 2 ? 148 : 296);
+  const int fb = B >= 8 ? 33 : (B >= 2 ? 132 : 264);
   fill_small_contours_kernel<<<dim3(fb, B), 256, smem_words * 4, st>>>(d_envs, smem_words);
   publish_kernel<<<B, 32, 0, st>>>(d_envs, 1);      // sticky: the host may poll it many steps later
   VLFM_CHECK_LAUNCH("vlfm_fill_small_holes_batch");

@@ -314,7 +314,7 @@ extern "C" int vlfm_proposal_scores(const float* d_q, const float* d_text, int B
     int rc = check_cuda(cudaFuncSetAttribute(proposal_scores_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "attr(proposal_scores)");
     if (rc) return rc; cfg = smem;
   }
-  int bx = (S + 7) / 8; if (bx > 296) bx = 296;
+  int bx = (S + 7) / 8; if (bx > 264) bx = 264;
   proposal_scores_kernel<<<dim3(bx, B), 256, smem, (cudaStream_t)stream>>>(d_q, d_text, S, T, D, d_scores);
   VLFM_CHECK_LAUNCH("proposal_scores_kernel");
   count_launch();
@@ -384,7 +384,7 @@ extern "C" int vlfm_contrastive_sigmoid(const float* d_hs, const float* d_text, 
     int rc = check_cuda(cudaFuncSetAttribute(contrastive_sigmoid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "attr(contrastive_sigmoid)");
     if (rc) return rc; cfg = smem;
   }
-  int bx = (Q + 7) / 8; if (bx > 148) bx = 148;
+  int bx = (Q + 7) / 8; if (bx > 132) bx = 132;
   contrastive_sigmoid_kernel<<<dim3(bx, B), 256, smem, (cudaStream_t)stream>>>(d_hs, d_text, Q, T, D, L, d_out);
   VLFM_CHECK_LAUNCH("contrastive_sigmoid_kernel");
   count_launch();

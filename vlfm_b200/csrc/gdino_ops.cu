@@ -386,7 +386,7 @@ extern "C" int vlfm_cast_f32_f16(const float* d_in, void* d_out16, long n, void*
   if (n == 0) return VLFM_OK;
   if (((uintptr_t)d_in & 15) || ((uintptr_t)d_out16 & 7)) { set_error("vlfm_cast_f32_f16: pointers must be 16 / 8 byte aligned"); return VLFM_E_INVALID; }
   const long n4 = n >> 2; const int tail = (int)(n & 3);
-  long blocks = (n4 + 255) / 256; if (blocks < 1) blocks = 1; if (blocks > 148 * 16) blocks = 148 * 16;
+  long blocks = (n4 + 255) / 256; if (blocks < 1) blocks = 1; if (blocks > 132 * 16) blocks = 132 * 16;
   cast_f32_f16_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((const float4*)d_in, (uint2*)d_out16, n4, d_in + 4 * n4,
                                                                           (__half*)d_out16 + 4 * n4, tail);
   VLFM_CHECK_LAUNCH("vlfm_cast_f32_f16");
@@ -427,7 +427,7 @@ extern "C" int vlfm_cast_addpos_f16(const float* d_x, const float* d_pos, void* 
   if (!d_x || (!d_out_x16 && !d_out_xp16) || n < 0 || (n & 3)) { set_error("vlfm_cast_addpos_f16: bad argument"); return VLFM_E_INVALID; }
   if (n == 0) return VLFM_OK;
   const long n4 = n >> 2;
-  long blocks = (n4 + 255) / 256; if (blocks > 148 * 16) blocks = 148 * 16;
+  long blocks = (n4 + 255) / 256; if (blocks > 132 * 16) blocks = 132 * 16;
   cast_addpos_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((const float4*)d_x, (const float4*)d_pos, (uint2*)d_out_x16, (uint2*)d_out_xp16, n4);
   VLFM_CHECK_LAUNCH("vlfm_cast_addpos_f16");
   count_launch();

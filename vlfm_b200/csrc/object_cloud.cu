@@ -1,4 +1,4 @@
-// Object point clouds on the GPU (sm_100a): mask erosion, masked unprojection in row-major order, DBSCAN largest cluster.
+// Object point clouds on the GPU (sm_90a): mask erosion, masked unprojection in row-major order, DBSCAN largest cluster.
 //
 // Reference: vlfm/mapping/object_point_cloud_map.py
 //   _extract_object_cloud :143-163   cv2.erode(mask*255, None, iterations=k) -> valid depth (0 -> 1, metres, float32)

@@ -1,4 +1,4 @@
-// Obstacle map: depth -> occupancy scatter and agent-radius dilation (sm_100a).
+// Obstacle map: depth -> occupancy scatter and agent-radius dilation (sm_90a).
 //
 // Reference path: vlfm/mapping/obstacle_map.py:86-109
 //   hole fill (:87-89, the hole_area_thresh == -1 form) -> metres (:92) -> mask (:93)
@@ -36,7 +36,7 @@ struct ObstDev {
 // few pixels that pass it.  `lazy_y`: T[9] == 0, so ez does not depend on the lateral coordinate (fma(0, py, acc) == acc);
 // `affine`: the last row of T is (0, 0, 0, 1), so the homogeneous divisor is exactly 1.0 and x / 1.0 == x.  Both hold for every
 // camera->episodic transform the policies build (xyz_yaw_to_tf_matrix); otherwise the general path runs.  FP64 divisions per pixel:
-// 5 -> ~1.05 (B200 retires 64 FP64 FMA/clk/SM; a division costs ~20 of them -- the kernel was division-bound).
+// 5 -> ~1.05 (an FP64 division costs about twenty FP64 FMAs -- the kernel was division-bound).
 // Float32 pre-screen of the height test (affine transforms only): the episodic height of the point evaluated in float32 is within
 // ~1e-5 m of the float64 value (|coordinates| < 100 m, four products); points farther than 5 mm outside the height band are
 // dropped before any float64 work -- the exact float64 test below still decides everything that is kept.  Nine pixels in ten stop here.

@@ -1,4 +1,4 @@
-// Non-GEMM operators of the GroundingDINO Swin-T backbone (sm_100a).
+// Non-GEMM operators of the GroundingDINO Swin-T backbone (sm_90a).
 // Reference call site: vlfm/vlm/grounding_dino.py:52-67 (to_tensor + ImageNet normalise, no resize,
 // then groundingdino's Swin-T backbone inside predict()).
 //   - swin_patch_im2col_kernel: uint8 HWC -> (x/255 - mean)/std (float32) -> fp16 rows of the 4x4/4
@@ -214,7 +214,7 @@ extern "C" int vlfm_swin_patch_im2col(const uint8_t* d_img, void* d_out, int B, 
   const int Hp = (H + 3) / 4, Wp = (W + 3) / 4;
   size_t n = (size_t)B * Hp * Wp * 48;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   swin_patch_im2col_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_img, (__half*)d_out, B, H, W, Hp, Wp, h_mean3[0], h_mean3[1],
                                                                      h_mean3[2], h_std3[0], h_std3[1], h_std3[2]);
   VLFM_CHECK_LAUNCH("swin_patch_im2col_kernel");
@@ -248,7 +248,7 @@ extern "C" int vlfm_swin_patch_merge(const float* d_x, float* d_out, int B, int 
   if (!d_x || !d_out || B < 1) { set_error("vlfm_swin_patch_merge: bad argument"); return VLFM_E_INVALID; }
   size_t n = (size_t)B * ((H + 1) / 2) * ((W + 1) / 2) * 4 * C;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   int rc = check_cuda(launch_pdl(swin_patch_merge_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, d_x, d_out, B, H, W, C),
                       "swin_patch_merge_kernel");
   if (rc) return rc;

@@ -1,4 +1,4 @@
-// Value-map FOV-cone projection + confidence-weighted fusion (sm_100a).
+// Value-map FOV-cone projection + confidence-weighted fusion (sm_90a).
 //
 // Reference path: vlfm/mapping/value_map.py:100-128 (update_map) =
 //   _process_local_data :221-286, _localize_new_data :288-319,
@@ -579,8 +579,8 @@ extern "C" int vlfm_value_update(const VlfmValueParams* p, int batch, const int3
   }
   int rpt = p->rows_per_tile;
   if (rpt <= 0) {
-    // aim for >= ~2 waves of 148 SMs while keeping the per-block blob load amortised
-    int tiles = (296 + batch - 1) / batch;
+    // aim for >= ~2 waves of 132 SMs while keeping the per-block blob load amortised
+    int tiles = (264 + batch - 1) / batch;
     if (tiles < 1) tiles = 1;
     if (tiles > d.R) tiles = d.R;
     rpt = (d.R + tiles - 1) / tiles;
@@ -600,7 +600,7 @@ extern "C" int vlfm_value_mask_unexplored(int G, int C, int batch, const int32_t
                                           float* d_value, const uint8_t* d_explored, void* stream) {
   if (!d_conf || !d_value || !d_explored || G < 1 || C < 1) { set_error("vlfm_value_mask_unexplored: bad argument"); return VLFM_E_INVALID; }
   if (batch <= 0) return VLFM_OK;
-  dim3 g(296, batch);
+  dim3 g(264, batch);
   value_mask_unexplored_kernel<<<g, 256, 0, (cudaStream_t)stream>>>(G, C, d_slot, d_conf, d_value, d_explored);
   VLFM_CHECK_LAUNCH("value_mask_unexplored_kernel");
   count_launch();

@@ -1,4 +1,4 @@
-// Non-GEMM operators of the BLIP-2 ITC forward (sm_100a):
+// Non-GEMM operators of the BLIP-2 ITC forward (sm_90a):
 //   - image preprocessing: PIL-exact antialiased bicubic resize (uint8, 22-bit fixed
 //     point, horizontal then vertical pass) + ToTensor + Normalize, written straight
 //     into the im2col layout of the 14x14/14 patch-embedding GEMM
@@ -606,7 +606,7 @@ extern "C" int vlfm_assemble_tokens(const float* d_patch, const float* d_cls, co
   if (!d_patch || !d_cls || !d_pos || !d_x) { set_error("vlfm_assemble_tokens: null argument"); return VLFM_E_INVALID; }
   size_t n = (size_t)B * T * D;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   assemble_tokens_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_patch, d_cls, d_pos, d_x, B, T, D);
   VLFM_CHECK_LAUNCH("assemble_tokens_kernel");
   count_launch();
@@ -683,10 +683,10 @@ extern "C" int vlfm_attention_f16(const void* d_q, const void* d_k, const void* 
   // few (batch, head, block) work items -> 32-row blocks with split keys (4-way when they fit one wave of 8-warp CTAs,
   // else 2-way); many -> 64-row blocks
   const long items = (long)B * heads * ((Nq + 31) / 32);
-  const bool big = items > 2 * 296;
+  const bool big = items > 2 * 264;
   static int kh4 = -1;
   if (kh4 < 0) { const char* e = getenv("VLFM_ATT_KH4"); kh4 = e ? atoi(e) : 1; }
-  const bool quad = !big && kh4 && items <= 296 && Nk >= 64;
+  const bool quad = !big && kh4 && items <= 264 && Nk >= 64;
   const int qblk = big ? 64 : 32;
   dim3 grid((Nq + qblk - 1) / qblk, heads, B);
   const size_t nkp = ((size_t)Nk + 15) & ~(size_t)15;
@@ -730,7 +730,7 @@ extern "C" int vlfm_attention_f32(const float* d_q, const float* d_k, const floa
   }
   // row groups: enough CTAs to cover the machine when few (image, head) pairs exist; every CTA stages K / V once
   int z = (Nq + 7) / 8;
-  while (z > 1 && (long)heads * B * z > 2 * 148) --z;
+  while (z > 1 && (long)heads * B * z > 2 * 132) --z;
   const dim3 grid(heads, B, z);
   cudaError_t e = hd == 32 ? launch_pdl(attention_f32_kernel<32>, grid, dim3(256), smem, (cudaStream_t)stream, d_q, d_k, d_v, (__half*)d_o_hi, (__half*)d_o_lo,
                                         ldq, ldk, ldv, ldo, Nq, Nk, scale)
@@ -744,7 +744,7 @@ extern "C" int vlfm_attention_f32(const float* d_q, const float* d_k, const floa
 extern "C" int vlfm_split_x2(const float* d_src, void* d_hi, void* d_lo, long long n, void* stream) {
   if (!d_src || !d_lo || n < 4 || (n & 3) || ((uintptr_t)d_src & 15) || ((uintptr_t)d_lo & 7) || ((uintptr_t)d_hi & 7)) {
     set_error("vlfm_split_x2: bad argument (n %% 4 == 0, aligned pointers)"); return VLFM_E_INVALID; }
-  long blocks = (n / 4 + 255) / 256; if (blocks > 148 * 8) blocks = 148 * 8;
+  long blocks = (n / 4 + 255) / 256; if (blocks > 132 * 8) blocks = 132 * 8;
   cudaError_t e = launch_pdl(split_x2_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, d_src, (__half*)d_hi, (__half*)d_lo, (long)(n / 4));
   { int rc = check_cuda(e, "split_x2_kernel"); if (rc) return rc; }
   count_launch();

@@ -56,9 +56,8 @@ class FullStep:
         self.acc = {k: 0.0 for k in self.names}
         self.n_front = 0
         self.nf = nf
-        # Three streams (detector | ITC | map update) are opt-in: VLFM_FULLSTEP_STREAMS=1.  Measured +5 % at 32 envs and +27 % at one
-        # env (profiles/r02_full_step_streams.txt), but two of three full bench.py runs with them stopped making progress at the end of
-        # round 2 (never reproduced in scripts/bench_full_step.py; not root-caused) -- the default is the one-stream sequence.
+        # Three streams (detector | ITC | map update) are opt-in: VLFM_FULLSTEP_STREAMS=1.  Full bench.py runs with them have stopped
+        # making progress (never reproduced in scripts/bench_full_step.py; not root-caused) -- the default is the one-stream sequence.
         self.serial = os.environ.get("VLFM_FULLSTEP_STREAMS", "0") != "1"
         self.sync_each = os.environ.get("VLFM_FULLSTEP_SERIAL", "0") == "1"   # diagnostic: device sync after every component
         self._streams = None

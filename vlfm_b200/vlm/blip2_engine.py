@@ -1,4 +1,4 @@
-"""BLIP-2 ITC forward on hand-written sm_100a kernels (through the C-ABI).
+"""BLIP-2 ITC forward on hand-written sm_90a kernels (through the C-ABI).
 
 Replaces what ``self.model({"image": img, "text_input": txt}, match_head="itc")`` does
 inside ``BLIP2ITM.cosine`` (vlfm/vlm/blip2itm.py:52) together with the preprocessing at
@@ -6,7 +6,7 @@ inside ``BLIP2ITM.cosine`` (vlfm/vlm/blip2itm.py:52) together with the preproces
 per-batch forward is captured once in a CUDA graph and replayed.
 
 Numerics: fp16 GEMM/attention operands (lavis runs the ViT under fp16 autocast too),
-fp32 accumulation (TMEM), fp32 residual stream, fp32 LayerNorm / softmax statistics.
+fp32 accumulation (registers), fp32 residual stream, fp32 LayerNorm / softmax statistics.
 """
 from __future__ import annotations
 

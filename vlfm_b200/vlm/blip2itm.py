@@ -93,7 +93,7 @@ class HashTokenizer:
 
 
 class BLIP2ITM:
-    """BLIP 2 Image-Text Matching model (ITC head), hand-written sm_100a forward."""
+    """BLIP 2 Image-Text Matching model (ITC head), hand-written sm_90a forward."""
 
     def __init__(self, name: str = "blip2_image_text_matching", model_type: str = "pretrain", device: Optional[Any] = None,
                  state_dict: Optional[Dict[str, torch.Tensor]] = None, dims: Optional[Blip2Dims] = None,

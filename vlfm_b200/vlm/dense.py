@@ -1,4 +1,4 @@
-"""Thin torch-tensor wrappers over the dense C-ABI entry points (csrc/gemm_tcgen05.cu ...)."""
+"""Thin torch-tensor wrappers over the dense C-ABI entry points (csrc/gemm_wgmma.cu ...)."""
 from __future__ import annotations
 
 from typing import Optional

@@ -3,7 +3,7 @@
 The module graph (fusion layers, deformable encoder, decoder, heads) is still HF's
 ``GroundingDinoForObjectDetection``; this file swaps its two hot primitives for the library's own kernels:
 
-* every ``nn.Linear``  -> ``TcLinear``: fp16 operands on the tcgen05 GEMM (csrc/gemm_tcgen05.cu), fp32 accumulate,
+* every ``nn.Linear``  -> ``TcLinear``: fp16 operands on the wgmma GEMM (csrc/gemm_wgmma.cu), fp32 accumulate,
   bias fused, fp32 out (the reference runs these in fp32 SIMT GEMMs: groundingdino ... nn.Linear);
 * ``MultiScaleDeformableAttention`` (groundingdino's ms_deform_attn_cuda.cu / HF's grid_sample fallback)
   -> ``vlfm_msda_forward`` (csrc/gdino_ops.cu).

@@ -17,7 +17,7 @@ which this class restates for inference on fully valid images (pixel_mask all on
     running it on all 6380 proposals, which is what the module graph does);
   * the heads run for the LAST decoder layer only (the other five are training-time auxiliary outputs).
 
-The encoder and decoder LAYERS are the HF layer objects whose sublayers ``gdino_accel`` replaced (tcgen05 GEMMs, fused deformable
+The encoder and decoder LAYERS are the HF layer objects whose sublayers ``gdino_accel`` replaced (wgmma GEMMs, fused deformable
 sampling, bi-attention); the stacks are sequenced here: the encoder loop feeds every layer the cached deformable reference points
 and the cached sine embedding of the text position ids (the module code rebuilds both per call / per layer), the decoder loop
 computes each layer's query position embedding with one kernel + the reference_points_head GEMMs and refines the reference points

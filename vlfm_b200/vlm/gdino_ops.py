@@ -1,5 +1,5 @@
 """Kernel interface of ``GdinoForward`` (vlm/gdino_forward.py) on the C-ABI library: every method is one or two launches of
-csrc/gdino_head.cu / gemm_tcgen05.cu / vit_ops.cu kernels over torch-owned buffers.  No torch arithmetic here."""
+csrc/gdino_head.cu / gemm_wgmma.cu / vit_ops.cu kernels over torch-owned buffers.  No torch arithmetic here."""
 from __future__ import annotations
 
 from typing import Optional

@@ -1,8 +1,8 @@
 """GroundingDINO behind the reference's class surface (vlfm/vlm/grounding_dino.py:23-85).
 
-The Swin-T backbone -- the dense contraction north_star names -- runs on the hand-written sm_100a kernels
+The Swin-T backbone -- the dense contraction north_star names -- runs on the hand-written sm_90a kernels
 (``SwinBackboneEngine``); every nn.Linear, the deformable encoder layers, the image<->text fusion layers and the decoder layers
-run on the library too (``gdino_accel``: tcgen05 GEMM, fused multi-scale deformable sampling, bi-attention).  The module graph
+run on the library too (``gdino_accel``: wgmma GEMM, fused multi-scale deformable sampling, bi-attention).  The module graph
 that sequences them is HF's ``GroundingDinoForObjectDetection`` (architecture-equivalent to groundingdino@eeba084); what is
 still PyTorch glue is listed in DESIGN.md section 7.  Post-processing restates groundingdino.util.inference.predict.
 """
@@ -105,7 +105,7 @@ class GroundingDINO:
         self._features = _Features()
         model.model.backbone.conv_encoder.model = self._features
         self.model = model.to(device).eval()
-        # feature enhancer / decoder: nn.Linear -> tcgen05 GEMM, deformable-attention sampling -> vlfm_msda_forward
+        # feature enhancer / decoder: nn.Linear -> wgmma GEMM, deformable-attention sampling -> vlfm_msda_forward
         self.accel = accelerate(self.model) if os.environ.get("VLFM_GDINO_ACCEL", "1") != "0" else {}
         # model-level glue (neck, proposal scoring, top-900 selection, heads) on the library's kernels; VLFM_GDINO_OWN_FORWARD=0 keeps
         # HF's GroundingDinoModel.forward for A/B comparisons

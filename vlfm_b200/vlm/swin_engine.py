@@ -1,9 +1,9 @@
-"""GroundingDINO's Swin-T backbone on hand-written sm_100a kernels (through the C-ABI).
+"""GroundingDINO's Swin-T backbone on hand-written sm_90a kernels (through the C-ABI).
 
 Reference: the image branch of ``groundingdino.util.inference.predict`` called at
 vlfm/vlm/grounding_dino.py:61-67, preceded by to_tensor + ImageNet normalise (:52-54; no
 resize -- the native 480x640 frame goes in).  GEMMs (patch embedding, QKV, projection, MLP,
-patch-merging reduction) run on the tcgen05 GEMM; LayerNorms on the shared LayerNorm kernel;
+patch-merging reduction) run on the wgmma GEMM; LayerNorms on the shared LayerNorm kernel;
 window attention / patch merging / patch im2col are csrc/swin_ops.cu.
 
 Weights use the HF ``SwinBackbone`` naming (the prefix inside a GroundingDINO checkpoint is
