@@ -153,8 +153,11 @@ int vlfm_fill_small_holes(const float* d_depth, int H, int W, double area_thresh
 #define VLFM_EPI_PARTIAL_F32 5   /* internal to vlfm_gemm_f16_resid_ln: split-K partial sums stored side by side */
 /* x[M,N] (fp32 residual stream) += A @ W^T + bias, then LayerNorm(x) -> d_out16 (fp16) and/or d_out32 (fp32, may
  * alias x for the post-LN Q-Former blocks).  BITWISE REPRODUCIBLE: when the tile plan splits K, the splits store their
- * partial sums in d_partials (>= splits * M * N floats, splits <= 8; no atomics) and the LayerNorm launch adds them to x in
- * split order before normalising; without d_partials (or when it is too small) the splits fall back to red.global.add into x.
+ * partial sums in d_partials (no atomics) and the LayerNorm launch adds them to x in K order before normalising.  Below one
+ * wave of 128 x 128 tiles the split is stream-K over one CTA per SM: (SMs + tiles - 1) slabs of 130 x 128 floats (66.5 KB);
+ * a smaller d_partials lowers the CTA count, and below tiles + 1 CTAs the GEMM runs unsplit.  Above one wave the splits are
+ * uniform (>= splits * M * N floats, splits <= 8); without d_partials (or when it is too small) they fall back to
+ * red.global.add into x.  Stream-K results depend on the SM count: bitwise reproducible across cards with the same count.
  * Replaces `x = x + proj(...)` followed by `layer_norm` in the BLIP-2 forward (blip2itm.py:52 through lavis).            */
 int vlfm_gemm_f16_resid_ln(const void* d_A, const void* d_W, const float* d_bias, float* d_x, int M, int N, int K,
                            int lda, int ldw, int ldx, const float* d_gamma, const float* d_beta, void* d_out16, int ld16,

@@ -31,9 +31,11 @@ def bench(M, Nn, K, epi):
     return e0.elapsed_time(e1) * 1e3 / (5 * N)
 
 sweep = len(sys.argv) > 1 and sys.argv[1] == "sweep"
-for (M, Nn, K, epi) in SHAPES:
+vit = 0.0
+for i, (M, Nn, K, epi) in enumerate(SHAPES):
     os.environ.pop("VLFM_GEMM_FORCE", None)
     base = bench(M, Nn, K, epi)
+    vit += base if i < 4 else 0.0
     line = f"{M}x{Nn}x{K} epi{epi}: model-plan {base:6.2f} us ({2*M*Nn*K/base/1e6:6.1f} TF)"
     if sweep:
         for bn in (128, 64, 32):
@@ -41,3 +43,6 @@ for (M, Nn, K, epi) in SHAPES:
                 os.environ["VLFM_GEMM_FORCE"] = f"{bn}:{sp}"
                 line += f" | {bn}:{sp}={bench(M, Nn, K, epi):.2f}"
     print(line, flush=True)
+# the four ViT-g layer GEMMs at batch 1 (qkv, proj, fc1, fc2) x 39 layers; proj and fc2 run here without a workspace (plain
+# residual epilogue), not through the stream-K path of vlfm_gemm_f16_resid_ln that the forward uses
+print(f"ViT-g batch-1 GEMMs x 39 layers: {vit * 39 / 1e3:.3f} ms", flush=True)

@@ -52,6 +52,28 @@ __device__ __forceinline__ void split_x2(float y, __half& hi, __half& lo) {
   hi = __float2half_rn(y);
   lo = __float2half_rn((y - __half2float(hi)) * X2_SCALE);
 }
+// Partial sums of a split residual GEMM, written by the GEMM and added to the residual stream by the LayerNorm launch
+// (layernorm_reduce_kernel).  Both sides take the layout from this struct, so they cannot disagree about it.
+//   splits > 0: uniform split-K.  Split s stores element (row, col) at s * stride + row * D + col.
+//   splits == 0: stream-K over 128 x 128 output tiles.  Tiles are ordered column block first (tile = n_blk * row_tiles + m_blk,
+//     so the row tiles that read one weight tile run next to each other) and the (tile, K-block) iterations of all tiles form
+//     one sequence, cut into `ctas` contiguous ranges of near-equal length.  CTA c stores the part of tile t it computed (a
+//     "segment") in slab c + t: ranges grow monotonically in both c and t, so no two segments share a slab, and
+//     ctas + tiles - 1 slabs hold them all.  A slab holds SK_SLAB_ROWS x SK_TILE floats: the tile's 128 rows, then the
+//     tail rows (M = 128 q + r, r <= 2) that the last row tile computes on CUDA cores.
+constexpr int SK_TILE = 128;
+constexpr int SK_SLAB_ROWS = SK_TILE + 2;
+constexpr long long SK_SLAB = (long long)SK_SLAB_ROWS * SK_TILE;   // floats
+struct SplitK {
+  int splits;
+  long long stride;                  // uniform split-K: floats between splits
+  int ctas, row_tiles, tiles, num_k;  // stream-K
+  // first iteration of CTA c (c = ctas: one past the last)
+  __host__ __device__ __forceinline__ int sk_begin(int c) const { return (int)((long long)c * tiles * num_k / ctas); }
+  // the CTA whose range holds iteration it
+  __host__ __device__ __forceinline__ int sk_owner(int it) const { return (int)(((long long)(it + 1) * ctas - 1) / ((long long)tiles * num_k)); }
+};
+
 __device__ __forceinline__ float ld_cg_f32(const float* p) { return __ldcg(p); }
 __device__ __forceinline__ uint32_t ld_cg_u32(const uint32_t* p) { return __ldcg(p); }
 

@@ -91,6 +91,17 @@ template <> struct Wgmma<64> {
         : VLFM_D16(d, 0), VLFM_D16(d, 16) : "l"(a), "l"(b), "r"(acc));
   }
 };
+template <> struct Wgmma<96> {
+  static __device__ __forceinline__ void mma(float (&d)[48], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+        : VLFM_D16(d, 0), VLFM_D16(d, 16), VLFM_D16(d, 32) : "l"(a), "l"(b), "r"(acc));
+  }
+};
 template <> struct Wgmma<128> {
   static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
     asm volatile(
@@ -122,8 +133,10 @@ struct GemmArgs {
   // every stage's TMA time on out-of-bounds zero fill.  Rows of the smem tile beyond the box keep whatever they held: row i of the
   // accumulator depends on row i of A only, and rows >= M are never stored.
   int a_box_rows;
+  SplitK sk;          // sk.ctas > 0: stream-K launch (1-D grid of sk.ctas CTAs, BN = SK_TILE); `out` is the slab workspace
 };
 constexpr int GEMM_TAIL_MAX = 2;
+static_assert(SK_SLAB_ROWS == BM + GEMM_TAIL_MAX && SK_TILE == BM, "stream-K slab = one 128 x 128 tile + its tail rows");
 constexpr int GEMM_TAIL_KMAX = 6144;   // K elements of one CTA's slice that fit the tail-row staging buffer
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
@@ -161,12 +174,11 @@ __device__ __forceinline__ void epilogue_store2(const GemmArgs& g, int row, int 
 }
 
 // Epilogue of one warp's 16 x BN accumulator slab, straight from the wgmma fragment.  `row0` = first row of the slab;
-// `sbias` = this tile's bias slice in shared memory (zero-filled past N / without bias).
+// `sbias` = this tile's bias slice in shared memory (zero-filled past N / without bias), added when `addb` (the first K split).
 template <int BN>
-__device__ __forceinline__ void epilogue_frag(const float (&acc)[BN / 2], int row0, int n_blk, const GemmArgs& g, bool split, const float* sbias) {
+__device__ __forceinline__ void epilogue_frag(const float (&acc)[BN / 2], int row0, int n_blk, const GemmArgs& g, bool split, bool addb, const float* sbias) {
   const int lane = threadIdx.x & 31;
   const int r_up = row0 + (lane >> 2), cq = (lane & 3) * 2;
-  const bool addb = blockIdx.z == 0;
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {
     const int cl = j * 8 + cq, n = n_blk * BN + cl;
@@ -184,6 +196,25 @@ __device__ __forceinline__ uint8_t* smem_align_1024(uint8_t* raw) {
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~(uintptr_t)1023);
 }
 
+// Stream-K segment store: this warp's 16 x BN slab of the accumulator (+ bias when the segment starts at K-block 0) into the
+// tile's slab of the workspace (SplitK in common.cuh).  Every column and row of the slab is written; the reduction reads those < N, < M.
+template <int BN>
+__device__ __forceinline__ void segment_store_frag(const float (&acc)[BN / 2], int row0, int n_blk, const GemmArgs& g, bool addb, float* slab) {
+  const int lane = threadIdx.x & 31;
+  const int r_up = row0 + (lane >> 2), cq = (lane & 3) * 2;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int cl = j * 8 + cq, n = n_blk * BN + cl;
+    const float b0 = (addb && g.bias && n < g.N) ? __ldg(g.bias + n) : 0.f, b1 = (addb && g.bias && n + 1 < g.N) ? __ldg(g.bias + n + 1) : 0.f;
+    *reinterpret_cast<float2*>(slab + (size_t)r_up * BN + cl) = make_float2(acc[4 * j] + b0, acc[4 * j + 1] + b1);
+    *reinterpret_cast<float2*>(slab + (size_t)(r_up + 8) * BN + cl) = make_float2(acc[4 * j + 2] + b0, acc[4 * j + 3] + b1);
+  }
+}
+
+// A CTA works through iterations [it0, it1) of a sequence of (output tile, K-block) pairs.  A grid launch gives it one tile
+// (blockIdx.x, blockIdx.y) and the K-blocks of split blockIdx.z.  A stream-K launch (g.sk.ctas > 0, 1-D grid) gives it a range
+// of the sequence of all tiles' K-blocks (SplitK in common.cuh), which may cover parts of two tiles: the producer streams straight
+// across the tile boundary, and the consumers finish a segment there (store it to the workspace, zero the accumulators) and go on.
 template <int BN, int STAGES>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmArgs g) {
@@ -198,11 +229,24 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 
   pdl_trigger();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_blk = blockIdx.x, m_blk = blockIdx.y;
-  const int kb_begin = blockIdx.z * g.kb_per_split;
-  const int num_k = min((g.K + BK - 1) / BK - kb_begin, g.kb_per_split);   // K-blocks of this split
-  const bool split = gridDim.z > 1;
-  const bool tail_cta = g.tail_rows > 0 && m_blk == (int)gridDim.y - 1;
+  const int nk = (g.K + BK - 1) / BK;
+  const bool sk = g.sk.ctas > 0;
+  const int it0 = sk ? g.sk.sk_begin(blockIdx.x) : blockIdx.z * g.kb_per_split;
+  const int it1 = sk ? g.sk.sk_begin(blockIdx.x + 1) : min(nk, it0 + g.kb_per_split);
+  const int last_m = sk ? g.sk.row_tiles - 1 : (int)gridDim.y - 1;
+  auto coords = [&](int it, int& m_blk, int& n_blk, int& kb) {
+    if (sk) { const int t = it / nk; kb = it - t * nk; m_blk = t % g.sk.row_tiles; n_blk = t / g.sk.row_tiles; }
+    else { kb = it; m_blk = blockIdx.y; n_blk = blockIdx.x; }
+  };
+  const bool split = !sk && gridDim.z > 1;
+  // tail rows (see GemmArgs): a grid CTA of the last row tile stages its K slice of them; a stream-K CTA whose range touches a
+  // tile of the last row stages the whole K (at most GEMM_TAIL_KMAX, checked by the host plan)
+  int m_first, n_first, kb_first;
+  coords(it0, m_first, n_first, kb_first);
+  // (tiles t of the last row: t % row_tiles == row_tiles - 1; floor((t + 1) / row_tiles) of them lie in [0, t])
+  const bool tail_cta = g.tail_rows > 0 &&
+      (sk ? ((it1 - 1) / nk + 1) / g.sk.row_tiles > (it0 / nk) / g.sk.row_tiles : m_first == last_m);
+  const int kb_lo = sk ? 0 : it0, kb_hi = sk ? nk : it1;
 
   if (warp == 0 && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
@@ -219,21 +263,26 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       // Weights do not depend on the predecessor kernel: start streaming the first STAGES W tiles BEFORE the
       // programmatic-dependency wait (hides the HBM/L2 latency of the first loads behind the predecessor's tail);
       // the matching A tiles (activations) are issued right after the wait and complete the same barriers.
-      const int pre = num_k < STAGES ? num_k : STAGES;
+      const int pre = min(it1 - it0, STAGES);
       const uint32_t a_tx = (uint32_t)g.a_box_rows * BK * 2;
-      for (int kb = 0; kb < pre; ++kb) {
-        mbar_expect_tx(full0 + 8 * kb, a_tx + B_BYTES);
-        tma_load_2d(smem_u32(sB + kb * B_BYTES), &tmB, (kb_begin + kb) * BK, n_blk * BN, full0 + 8 * kb);
+      int m_blk, n_blk, kb;
+      for (int i = 0; i < pre; ++i) {
+        coords(it0 + i, m_blk, n_blk, kb);
+        mbar_expect_tx(full0 + 8 * i, a_tx + B_BYTES);
+        tma_load_2d(smem_u32(sB + i * B_BYTES), &tmB, kb * BK, n_blk * BN, full0 + 8 * i);
       }
       pdl_wait();
-      for (int kb = 0; kb < pre; ++kb)
-        tma_load_2d(smem_u32(sA + kb * A_BYTES), &tmA, (kb_begin + kb) * BK, m_blk * BM, full0 + 8 * kb);
+      for (int i = 0; i < pre; ++i) {
+        coords(it0 + i, m_blk, n_blk, kb);
+        tma_load_2d(smem_u32(sA + i * A_BYTES), &tmA, kb * BK, m_blk * BM, full0 + 8 * i);
+      }
       int s = pre == STAGES ? 0 : pre; uint32_t ph = pre == STAGES ? 1 : 0;
-      for (int kb = pre; kb < num_k; ++kb) {
+      for (int it = it0 + pre; it < it1; ++it) {
+        coords(it, m_blk, n_blk, kb);
         mbar_wait(empty0 + 8 * s, ph ^ 1);
         mbar_expect_tx(full0 + 8 * s, a_tx + B_BYTES);
-        tma_load_2d(smem_u32(sA + s * A_BYTES), &tmA, (kb_begin + kb) * BK, m_blk * BM, full0 + 8 * s);
-        tma_load_2d(smem_u32(sB + s * B_BYTES), &tmB, (kb_begin + kb) * BK, n_blk * BN, full0 + 8 * s);
+        tma_load_2d(smem_u32(sA + s * A_BYTES), &tmA, kb * BK, m_blk * BM, full0 + 8 * s);
+        tma_load_2d(smem_u32(sB + s * B_BYTES), &tmB, kb * BK, n_blk * BN, full0 + 8 * s);
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
@@ -241,21 +290,20 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     // ---- consumers: warpgroup wg owns rows [64 * wg, +64) of the tile, warp wq of it rows [16 * wq, +16) of those
     const int wg = (warp >> 2) - 1, wq = warp & 3;
     const int et = threadIdx.x - (GEMM_THREADS - GEMM_CONSUMERS);
-    const int wg_row0 = m_blk * BM + wg * 64;
-    const bool active = wg_row0 < g.M;      // a warpgroup whose rows are all past M (M <= 64) issues no MMA
-    // bias is a weight (no dependency on the predecessor): stage this tile's slice while the first loads are in flight
-    if (et < BN) { const int n = n_blk * BN + et; sbias[et] = (g.bias && n < g.N) ? __ldg(g.bias + n) : 0.f; }
+    // a warpgroup whose rows are all past M issues no MMA (a stream-K range may span row tiles: there both always compute)
+    const bool active = sk || m_first * BM + wg * 64 < g.M;
+    // bias is a weight (no dependency on the predecessor): stage this tile's slice while the first loads are in flight.
+    // (Stream-K segments read it from global memory: their tiles change along the range.)
+    if (!sk && et < BN) { const int n = n_first * BN + et; sbias[et] = (g.bias && n < g.N) ? __ldg(g.bias + n) : 0.f; }
     asm volatile("bar.sync 1, 256;" ::: "memory");   // the eight consumer warps only
     pdl_wait();          // residual stream / output buffers of the predecessor are visible
     // ---- tail rows on CUDA cores: thread = (feature f of this tile, K half hk); W from the 128B-swizzled stage
     const int f = et >> 1, hk = et & 1;
     float tacc[GEMM_TAIL_MAX];
-#pragma unroll
-    for (int r = 0; r < GEMM_TAIL_MAX; ++r) tacc[r] = 0.f;
     __half* sx = reinterpret_cast<__half*>(sbias + BN);
-    const int kslice = num_k * BK, kbase = kb_begin * BK;
+    const int kslice = (kb_hi - kb_lo) * BK, kbase = kb_lo * BK;
     if (tail_cta) {
-      // stage this CTA's K slice of the tail rows once (global latency must not sit between "stage full" and "stage released")
+      // stage the K slice of the tail rows once (global latency must not sit between "stage full" and "stage released")
       for (int i = et; i < g.tail_rows * (kslice >> 3); i += GEMM_CONSUMERS) {
         const int r = i / (kslice >> 3), c8 = (i - r * (kslice >> 3)) << 3;
         uint4 xv = make_uint4(0u, 0u, 0u, 0u);
@@ -266,7 +314,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     }
     if (!active) {     // keep the ring turning for the other warpgroup: take every stage and hand it straight back
       int s = 0; uint32_t ph = 0;
-      for (int kb = 0; kb < num_k; ++kb) {
+      for (int it = it0; it < it1; ++it) {
         mbar_wait(full0 + 8 * s, ph);
         __syncwarp();
         if (lane == 0) mbar_arrive(empty0 + 8 * s);
@@ -278,17 +326,28 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     int s = 0; uint32_t ph = 0;
-    for (int kb = 0; kb < num_k; ++kb) {
+    bool held = false;       // the stage before s is still held (its wgmma group may be in flight)
+    bool addb = false;       // the current segment starts at K-block 0: it carries the bias
+    for (int it = it0; it < it1; ++it) {
+      int m_blk, n_blk, kb;
+      coords(it, m_blk, n_blk, kb);
+      const bool seg_first = it == it0 || kb == 0, seg_last = it + 1 == it1 || kb + 1 == nk;
+      const bool tail_seg = tail_cta && m_blk == last_m;
+      if (seg_first) {
+        addb = kb == 0;
+#pragma unroll
+        for (int r = 0; r < GEMM_TAIL_MAX; ++r) tacc[r] = 0.f;
+      }
       mbar_wait(full0 + 8 * s, ph);
       const uint32_t a0 = smem_u32(sA + s * A_BYTES) + (uint32_t)wg * (64 * BK * 2), b0 = smem_u32(sB + s * B_BYTES);
       wg_fence();
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k)
-        Wgmma<BN>::mma(acc, wgmma_desc_k128(a0 + k * 32), wgmma_desc_k128(b0 + k * 32), (kb > 0 || k > 0) ? 1u : 0u);
+        Wgmma<BN>::mma(acc, wgmma_desc_k128(a0 + k * 32), wgmma_desc_k128(b0 + k * 32), (!seg_first || k > 0) ? 1u : 0u);
       wg_commit();
-      if (tail_cta && f < BN) {     // overlaps the MMAs just issued
+      if (tail_seg && f < BN) {     // overlaps the MMAs just issued
         const uint8_t* wrow = sB + (size_t)s * B_BYTES + (size_t)f * 128;
-        const int k0 = kb * BK + hk * 32;                    // offset inside the staged slice
+        const int k0 = (kb - kb_lo) * BK + hk * 32;          // offset inside the staged slice
         uint4 wv[4];
 #pragma unroll
         for (int c = 0; c < 4; ++c) wv[c] = *reinterpret_cast<const uint4*>(wrow + (((hk * 4 + c) ^ (f & 7)) << 4));
@@ -314,38 +373,55 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       }
       // the group issued one K-block ago has retired once at most one is pending: its stage goes back to the producer
       wg_wait<1>();
-      if (kb > 0) {
+      if (held) {
         __syncwarp();
         if (lane == 0) mbar_arrive(empty0 + 8 * (s == 0 ? STAGES - 1 : s - 1));
       }
-      if (++s == STAGES) { s = 0; ph ^= 1; }
-    }
-    wg_wait<0>();
-    if (tail_cta) {
+      held = true;
+      if (seg_last) {
+        wg_wait<0>();
+        if (sk) {            // this stage is done with: hand it back before the segment's stores
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty0 + 8 * s);
+          held = false;
+        }
+        float* slab = sk ? reinterpret_cast<float*>(g.out) + (size_t)(blockIdx.x + n_blk * g.sk.row_tiles + m_blk) * SK_SLAB : nullptr;
+        if (tail_seg) {
 #pragma unroll
-      for (int r = 0; r < GEMM_TAIL_MAX; ++r) tacc[r] += __shfl_xor_sync(0xffffffffu, tacc[r], 1);
-      const int n = n_blk * BN + f;
-      if (hk == 0 && f < BN && n < g.N) {
+          for (int r = 0; r < GEMM_TAIL_MAX; ++r) tacc[r] += __shfl_xor_sync(0xffffffffu, tacc[r], 1);
+          const int n = n_blk * BN + f;
+          if (hk == 0 && f < BN && (sk || n < g.N)) {
 #pragma unroll
-        for (int r = 0; r < GEMM_TAIL_MAX; ++r) {
-          if (r < g.tail_rows) {
-            float v = tacc[r] + (blockIdx.z == 0 ? sbias[f] : 0.f);
-            const size_t o = (size_t)(g.tail_row0 + r) * g.ldo + n;
-            if (g.epi == VLFM_EPI_BIAS_F16 || g.epi == VLFM_EPI_BIAS_GELU_F16 || g.epi == VLFM_EPI_BIAS_RELU_F16) {
-              if (g.epi == VLFM_EPI_BIAS_GELU_F16) v = gelu_erf(v);
-              else if (g.epi == VLFM_EPI_BIAS_RELU_F16) v = fmaxf(v, 0.f);
-              reinterpret_cast<__half*>(g.out)[o] = __float2half_rn(v);
-            } else {
-              const bool partial = (g.epi == VLFM_EPI_PARTIAL_F32);
-              float* po = reinterpret_cast<float*>(g.out) + (partial ? (size_t)blockIdx.z * (size_t)g.split_stride : 0) + o;
-              if (split && !partial) atomicAdd(po, v);
-              else *po = (g.epi == VLFM_EPI_BIAS_RESID_F32) ? *po + v : v;
+            for (int r = 0; r < GEMM_TAIL_MAX; ++r) {
+              if (r < g.tail_rows) {
+                if (sk) {
+                  slab[(size_t)(BM + r) * BN + f] = tacc[r] + ((addb && g.bias && n < g.N) ? __ldg(g.bias + n) : 0.f);
+                  continue;
+                }
+                float v = tacc[r] + (addb ? sbias[f] : 0.f);
+                const size_t o = (size_t)(g.tail_row0 + r) * g.ldo + n;
+                if (g.epi == VLFM_EPI_BIAS_F16 || g.epi == VLFM_EPI_BIAS_GELU_F16 || g.epi == VLFM_EPI_BIAS_RELU_F16) {
+                  if (g.epi == VLFM_EPI_BIAS_GELU_F16) v = gelu_erf(v);
+                  else if (g.epi == VLFM_EPI_BIAS_RELU_F16) v = fmaxf(v, 0.f);
+                  reinterpret_cast<__half*>(g.out)[o] = __float2half_rn(v);
+                } else {
+                  const bool partial = (g.epi == VLFM_EPI_PARTIAL_F32);
+                  float* po = reinterpret_cast<float*>(g.out) + (partial ? (size_t)blockIdx.z * (size_t)g.split_stride : 0) + o;
+                  if (split && !partial) atomicAdd(po, v);
+                  else *po = (g.epi == VLFM_EPI_BIAS_RESID_F32) ? *po + v : v;
+                }
+              }
             }
           }
         }
+        if (sk) {
+          segment_store_frag<BN>(acc, wg * 64 + wq * 16, n_blk, g, addb, slab);
+        } else {
+          epilogue_frag<BN>(acc, m_blk * BM + wg * 64 + wq * 16, n_blk, g, split, addb, sbias);
+        }
       }
+      if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-    epilogue_frag<BN>(acc, wg_row0 + wq * 16, n_blk, g, split, sbias);
   }
 }
 
@@ -465,7 +541,7 @@ gemm_f16x2_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
     wg_wait<0>();
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = fmaf(corr[i], 1.f / X2_SCALE, acc[i]);
-    epilogue_frag<BN>(acc, wg_row0 + wq * 16, n_blk, g, split, sbias);
+    epilogue_frag<BN>(acc, wg_row0 + wq * 16, n_blk, g, split, blockIdx.z == 0, sbias);
   }
 }
 
@@ -519,6 +595,7 @@ static int launch_gemm(const CUtensorMap& ta, const void* W, int ldw, const Gemm
   }
   const int num_k = (g.K + BK - 1) / BK;
   dim3 grid((g.N + BN - 1) / BN, g.tail_rows > 0 ? g.M / BM : (g.M + BM - 1) / BM, (num_k + g.kb_per_split - 1) / g.kb_per_split);
+  if (g.sk.ctas > 0) grid = dim3(g.sk.ctas);
   rc = check_cuda(launch_pdl(gemm_f16_wgmma_kernel<BN, STAGES>, grid, dim3(GEMM_THREADS), smem, st, ta, tb, g), "gemm_f16_wgmma_kernel");
   if (rc) return rc;
   count_launch();
@@ -553,7 +630,7 @@ static int launch_gemm_x2(const CUtensorMap& ta, const CUtensorMap& tal, const v
 using namespace vlfm;
 
 static int gemm_dispatch(const void* d_A, const void* d_W, int M, int N, int K, int lda, int ldw, GemmArgs g, void* stream, float* d_partials,
-                         size_t partial_bytes, int* splits_out);
+                         size_t partial_bytes, SplitK* layout);
 
 // SMs of the current device (one GEMM CTA per SM): the launch plans size a wave by it.  132 on an H100 SXM.
 static int sm_count() {
@@ -572,18 +649,19 @@ extern "C" int vlfm_gemm_f16(const void* d_A, const void* d_W, const float* d_bi
   return gemm_dispatch(d_A, d_W, M, N, K, lda, ldw, g, stream, nullptr, 0, nullptr);
 }
 
+// Stream-K: the least number of K-blocks a CTA works through.  Below it the fixed cost of a CTA (barrier set-up, the first
+// loads, one or two segment stores of 66 KB) outweighs the K-blocks it takes off the other CTAs.
+constexpr int SK_MIN_ITERS = 3;
+
 static int gemm_dispatch(const void* d_A, const void* d_W, int M, int N, int K, int lda, int ldw, GemmArgs g, void* stream, float* d_partials,
-                         size_t partial_bytes, int* splits_out) {
-  if (splits_out) *splits_out = 1;
+                         size_t partial_bytes, SplitK* layout) {
+  if (layout) *layout = SplitK{1, 0};
   const int epilogue = g.epi;
   CUtensorMap ta;
   g.a_box_rows = M <= 32 ? 32 : (M <= 64 ? 64 : BM);
   int rc = make_map(&ta, d_A, M, K, lda, g.a_box_rows);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  // Tile / split-K plan from a small cost model (us): waves x (fixed + bytes a CTA must pull / its share of
-  // the L2->SM bandwidth).  Never spill into a second wave for a handful of CTAs; split K only for the
-  // fp32 residual epilogue (the splits store partial sums the LayerNorm launch reduces, or red.add without it).
   const int mt = (M + BM - 1) / BM, num_k = (K + BK - 1) / BK;
   const int sms = sm_count();
   // M = 128*q + r with a tiny remainder (ViT: 257 tokens = 2*128 + 1): launch q row tiles only; the last tile's CTAs compute
@@ -593,66 +671,102 @@ static int gemm_dispatch(const void* d_A, const void* d_W, int M, int N, int K, 
   if (tail_on < 0) { const char* e = getenv("VLFM_GEMM_TAIL"); tail_on = (e && e[0] == '0') ? 0 : 1; }
   const int rem = M % BM;
   const bool tail = tail_on && M > BM && rem >= 1 && rem <= GEMM_TAIL_MAX && num_k * BK <= GEMM_TAIL_KMAX;
+  const int rt = tail ? M / BM : mt;     // row tiles launched
+  const char* force = getenv("VLFM_GEMM_FORCE");   // development sweep: "bn:splits" (grid launches only)
+  const bool resid = epilogue == VLFM_EPI_BIAS_RESID_F32;
+  const int tiles128 = rt * ((N + BM - 1) / BM);
   int best_bn = 128, best_s = 1;
-  double best_t = 1e30;
-  bool best_tail = false;
-  // Cost model:  t = waves * (c0 + K-blocks per CTA * per_kb),  per_kb = max(pipeline floor, CTAs * KB per K-block / chip L2->SM rate),
-  //   c0 = prologue + epilogue per tile width, + split-K stores, + the tail-row work.  One CTA per SM (H100: 132).  The rate
-  //   (5.5 TB/s) and the floor / c0 terms are estimates for H100, not fitted to measurements on it.
-  const int bns[3] = {128, 64, 32};
-  for (int tm = 0; tm < (tail ? 2 : 1); ++tm) {
-    const bool use_tail = tail && tm == 0;
-    const int mte = use_tail ? M / BM : mt;
-    for (int bi = 0; bi < 3; ++bi) {
-      const int bn = bns[bi], nt = (N + bn - 1) / bn;
-      int smax = (epilogue == VLFM_EPI_BIAS_RESID_F32) ? num_k / 4 : 1;
-      static int smax_cap = -1;
-      if (smax_cap < 0) { const char* e = getenv("VLFM_GEMM_SMAX"); smax_cap = e ? atoi(e) : 8; if (smax_cap < 1 || smax_cap > 8) smax_cap = 8; }
-      if (smax < 1) smax = 1;
-      if (smax > smax_cap) smax = smax_cap;
-      for (int sp = 1; sp <= smax; ++sp) {
-        const double ctas = (double)mte * nt * sp;
-        const int kb = (num_k + sp - 1) / sp;
-        const double waves = (double)(long)((ctas + sms - 1) / sms);
-        const double active = ctas < sms ? ctas : sms;
-        const double kb_kbytes = (double)(128 + bn) * 128 / 1024.0;
-        double per_kb = active * kb_kbytes / 5500.0;
-        if (per_kb < 0.33) per_kb = 0.33;
-        double c0 = bn == 128 ? 3.8 + 0.22 * sp : (bn == 64 ? 3.0 : 2.6) + (sp > 1 ? 0.1 * sp : 0.0);
-        if (use_tail) c0 += bn == 128 ? 0.9 : 0.3;
-        const double t = waves * (c0 + kb * per_kb);
-        if (t < best_t) { best_t = t; best_bn = bn; best_s = sp; best_tail = use_tail; }
+  bool best_tail = tail;
+  if (tiles128 < sms && resid && d_partials && !force) {
+    // Less than one wave of 128 x 128 tiles, and a workspace: stream-K.  Every SM gets the same number of K-blocks (+-1) of the
+    // tiles' K-block sequence (SplitK in common.cuh); the LayerNorm launch adds the segments of each tile in K order.
+    const long long iters = (long long)tiles128 * num_k;
+    long long P = iters / SK_MIN_ITERS;
+    if (P > sms) P = sms;
+    const long long fit = (long long)(partial_bytes / (SK_SLAB * 4)) - (tiles128 - 1);
+    if (P > fit) P = fit;
+    if (P > tiles128) {
+      g.sk = SplitK{0, 0, (int)P, rt, tiles128, num_k};
+      g.out = d_partials;
+      if (tail) { g.a_tail = (const __half*)d_A + (size_t)rt * BM * lda; g.lda = lda; g.tail_rows = rem; g.tail_row0 = rt * BM; }
+      if (layout) *layout = g.sk;
+      return launch_gemm<128, 6>(ta, d_W, ldw, g, st);
+    }
+  }
+  if (tiles128 <= sms && !resid) {
+    // Less than one wave, no split: the tile width that leaves the busiest SM the fewest columns, ceil(tiles / SMs) * BN
+    // (the wider tile on a tie: fewer A re-reads).  ViT-g at batch 1: qkv BN 64 (132 CTAs), fc1 BN 96 (128 CTAs).
+    const int bns[4] = {128, 96, 64, 32};
+    long long best = -1;
+    for (int bn : bns) {
+      const long long tl = (long long)rt * ((N + bn - 1) / bn), cols = (tl + sms - 1) / sms * bn;
+      if (best < 0 || cols < best) { best = cols; best_bn = bn; }
+    }
+  } else {
+    // Tile / split-K plan from a small cost model (us): waves x (fixed + bytes a CTA must pull / its share of the L2->SM
+    // bandwidth).  Never spill into a second wave for a handful of CTAs; split K only for the fp32 residual epilogue (red.add,
+    // or without a workspace above it partial sums the LayerNorm launch reduces), and not at all for residual calls with a
+    // workspace below a wave (those are stream-K, or unsplit when the workspace is too small).
+    double best_t = 1e30;
+    // Cost model:  t = waves * (c0 + K-blocks per CTA * per_kb),  per_kb = max(pipeline floor, CTAs * KB per K-block / chip L2->SM rate),
+    //   c0 = prologue + epilogue per tile width, + split-K stores, + the tail-row work.  One CTA per SM (H100: 132).  The rate
+    //   (5.5 TB/s) and the floor / c0 terms are estimates for H100, not fitted to measurements on it.
+    const int bns[3] = {128, 64, 32};
+    for (int tm = 0; tm < (tail ? 2 : 1); ++tm) {
+      const bool use_tail = tail && tm == 0;
+      const int mte = use_tail ? M / BM : mt;
+      for (int bi = 0; bi < 3; ++bi) {
+        const int bn = bns[bi], nt = (N + bn - 1) / bn;
+        int smax = resid && !(d_partials && tiles128 < sms) ? num_k / 4 : 1;
+        if (smax < 1) smax = 1;
+        if (smax > 8) smax = 8;
+        for (int sp = 1; sp <= smax; ++sp) {
+          const double ctas = (double)mte * nt * sp;
+          const int kb = (num_k + sp - 1) / sp;
+          const double waves = (double)(long)((ctas + sms - 1) / sms);
+          const double active = ctas < sms ? ctas : sms;
+          const double kb_kbytes = (double)(128 + bn) * 128 / 1024.0;
+          double per_kb = active * kb_kbytes / 5500.0;
+          if (per_kb < 0.33) per_kb = 0.33;
+          double c0 = bn == 128 ? 3.8 + 0.22 * sp : (bn == 64 ? 3.0 : 2.6) + (sp > 1 ? 0.1 * sp : 0.0);
+          if (use_tail) c0 += bn == 128 ? 0.9 : 0.3;
+          const double t = waves * (c0 + kb * per_kb);
+          if (t < best_t) { best_t = t; best_bn = bn; best_s = sp; best_tail = use_tail; }
+        }
       }
     }
   }
-  if (const char* f = getenv("VLFM_GEMM_FORCE")) {   // development sweep: "bn:splits"
+  if (force) {
     int fb = 0, fs = 0;
-    if (sscanf(f, "%d:%d", &fb, &fs) == 2 && (fb == 128 || fb == 64 || fb == 32) && fs >= 1) {
+    if (sscanf(force, "%d:%d", &fb, &fs) == 2 && (fb == 128 || fb == 96 || fb == 64 || fb == 32) && fs >= 1) {
       best_bn = fb;
-      best_s = (epilogue == VLFM_EPI_BIAS_RESID_F32) ? (fs > num_k ? num_k : fs) : 1;
+      best_s = resid ? (fs > num_k ? num_k : fs) : 1;
     }
   }
   g.kb_per_split = (num_k + best_s - 1) / best_s;
   if (best_tail) { g.a_tail = (const __half*)d_A + (size_t)(M / BM) * BM * lda; g.lda = lda; g.tail_rows = rem; g.tail_row0 = (M / BM) * BM; }
   // deterministic split-K: the splits store their partial sums side by side and the caller reduces them in a fixed order
   const int launched_splits = (num_k + g.kb_per_split - 1) / g.kb_per_split;      // grid.z (can be below best_s when num_k is small)
-  if (d_partials && launched_splits > 1 && epilogue == VLFM_EPI_BIAS_RESID_F32 && (size_t)launched_splits * (size_t)M * (size_t)N * 4 <= partial_bytes) {
+  if (d_partials && launched_splits > 1 && resid && (size_t)launched_splits * (size_t)M * (size_t)N * 4 <= partial_bytes) {
     g.epi = VLFM_EPI_PARTIAL_F32; g.out = d_partials; g.ldo = N; g.split_stride = (long long)M * N;
-    if (splits_out) *splits_out = launched_splits;
+    if (layout) *layout = SplitK{launched_splits, (long long)M * N};
   }
   if (best_bn == 128) return launch_gemm<128, 6>(ta, d_W, ldw, g, st);
+  if (best_bn == 96) return launch_gemm<96, 7>(ta, d_W, ldw, g, st);
   if (best_bn == 64) return launch_gemm<64, 8>(ta, d_W, ldw, g, st);
   return launch_gemm<32, 8>(ta, d_W, ldw, g, st);
 }
 
 extern "C" int vlfm_layernorm(const float* d_x, const float* d_gamma, const float* d_beta, void* d_out16, float* d_out32,
                    int rows, int D, int ldx, int ldo16, int ldo32, float eps, void* stream);
-extern "C" int vlfm_layernorm_reduce(float* d_x, const float* d_partials, int splits, long long split_stride, const float* d_gamma,
-                                     const float* d_beta, void* d_out16, float* d_out32, int rows, int D, int ldx, int ldo16, int ldo32,
-                                     float eps, void* stream);
+namespace vlfm {
+int layernorm_reduce_impl(float* d_x, const float* d_partials, const SplitK& sk, const float* d_gamma, const float* d_beta, void* d_out16,
+                          void* d_out16_lo, float* d_out32, int rows, int D, int ldx, int ldo16, int ldo32, float eps, void* stream);
+}
 
-// x += A @ W^T + bias ; out = LayerNorm(x) -- bitwise reproducible: when the plan splits K, the splits store their partial sums
-// in d_partials (no atomics) and the LayerNorm kernel adds them to x in split order before normalising; an unsplit GEMM adds
+// x += A @ W^T + bias ; out = LayerNorm(x) -- bitwise reproducible: when the plan splits K (stream-K below a wave of tiles, uniform
+// splits above), the splits store their partial sums in d_partials (no atomics) and the LayerNorm kernel adds them to x in K order
+// before normalising; an unsplit GEMM adds
 // into x directly (one writer per element).  (Round 1 reduced the splits with red.global.add: the order of arrival varied from run
 // to run and the 39-layer residual stream amplified the last-bit differences to ~6e-5 on the cosine.)
 extern "C" int vlfm_gemm_f16_resid_ln(const void* d_A, const void* d_W, const float* d_bias, float* d_x, int M, int N, int K,
@@ -663,10 +777,10 @@ extern "C" int vlfm_gemm_f16_resid_ln(const void* d_A, const void* d_W, const fl
   if ((K & 7) || (lda & 7) || (ldw & 7) || (ldx & 7) || (N & 3) || (ld16 & 3) || (ld32 & 3) || ((uintptr_t)d_A & 15) || ((uintptr_t)d_W & 15) ||
       ((uintptr_t)d_x & 15) || ((uintptr_t)d_partials & 15)) { set_error("vlfm_gemm_f16_resid_ln: alignment (K, strides %% 8; N %% 4; 16-byte pointers)"); return VLFM_E_INVALID; }
   GemmArgs g{d_bias, d_x, M, N, K, ldx, VLFM_EPI_BIAS_RESID_F32, (K + BK - 1) / BK, 0, nullptr, 0, 0, 0, nullptr, BM};
-  int splits = 1;
-  int rc = gemm_dispatch(d_A, d_W, M, N, K, lda, ldw, g, stream, d_partials, partial_bytes, &splits);
+  SplitK layout;
+  int rc = gemm_dispatch(d_A, d_W, M, N, K, lda, ldw, g, stream, d_partials, partial_bytes, &layout);
   if (rc) return rc;
-  if (splits > 1) return vlfm_layernorm_reduce(d_x, d_partials, splits, (long long)M * N, d_gamma, d_beta, d_out16, d_out32, M, N, ldx, ld16, ld32, eps, stream);
+  if (layout.splits != 1) return layernorm_reduce_impl(d_x, d_partials, layout, d_gamma, d_beta, d_out16, nullptr, d_out32, M, N, ldx, ld16, ld32, eps, stream);
   return vlfm_layernorm(d_x, d_gamma, d_beta, d_out16, d_out32, M, N, ldx, ld16, ld32, eps, stream);
 }
 

@@ -140,15 +140,16 @@ layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma, c
   }
 }
 
-// x_row += sum_s partial[s][row] (s = 0 .. splits-1, in that order), written back; then LayerNorm of the updated row.
-// The deterministic reduction of a split-K residual GEMM (vlfm_gemm_f16_resid_ln).  One 128-thread block per row (<= 3 float4
-// per thread), the partial sums of up to four splits are loaded before the first add: with a warp per row and a runtime loop
-// over the splits (first version) the kernel paid one L2 round trip per split (9.5 us for 8 splits at 257 x 1408; the
-// deterministic forward was 12 % slower than the red.add one).  The adds stay in split order -> bitwise reproducible.
+// x_row += the partial sums of a split residual GEMM (layout: SplitK in common.cuh), added in K order and written back; then
+// LayerNorm of the updated row.  The deterministic reduction of vlfm_gemm_f16_resid_ln / vlfm_gemm_f16x2_resid_ln: the adds
+// always run in the same order -> bitwise reproducible.  Each thread owns one float4 of the row, so it reads the slabs of one
+// output tile (stream-K: the segments of that tile, their number differs between column blocks); the loads of up to four slabs
+// are issued before the first add: with a warp per row and a runtime loop over the splits (first version) the kernel paid one
+// L2 round trip per split (9.5 us for 8 splits at 257 x 1408; the deterministic forward was 12 % slower than the red.add one).
 // One float4 per thread, D/4 threads per row (<= 384): 11 warps per 1408-wide row keep ~20 warps per SM in flight (the 128-thread
 // version ran at 10 % occupancy, 6.5-8.5 us per launch, 78 launches per ViT forward).
 __global__ void __launch_bounds__(384)
-layernorm_reduce_kernel(float* x, const float* __restrict__ partials, int splits, long long split_stride,
+layernorm_reduce_kernel(float* x, const float* __restrict__ partials, SplitK sk,
                         const float* __restrict__ gamma, const float* __restrict__ beta, __half* __restrict__ out16,
                         float* out32, int rows, int D, int ldx, int ldo16, int ldo32, float eps, __half* __restrict__ out16_lo) {   // out32 may alias x (post-LN blocks)
   pdl_trigger();
@@ -158,19 +159,29 @@ layernorm_reduce_kernel(float* x, const float* __restrict__ partials, int splits
   const bool on = t < D4;
   const float4 g = on ? __ldg(reinterpret_cast<const float4*>(gamma) + t) : make_float4(0, 0, 0, 0);   // parameters do not depend on
   const float4 bt = on ? __ldg(reinterpret_cast<const float4*>(beta) + t) : make_float4(0, 0, 0, 0);   // the predecessor kernel
+  // slabs [s0, s1) hold this thread's four columns, at partials + s * stride + off
+  int s0 = 0, s1 = sk.splits;
+  long long stride = sk.stride, off = (long long)row * D + 4 * t;
+  if (sk.splits == 0) {
+    const int m = min(row / SK_TILE, sk.row_tiles - 1), nb = (4 * t) / SK_TILE, tile = nb * sk.row_tiles + m;
+    s0 = sk.sk_owner(tile * sk.num_k) + tile;
+    s1 = sk.sk_owner((tile + 1) * sk.num_k - 1) + tile + 1;
+    stride = SK_SLAB;
+    off = (long long)(row - m * SK_TILE) * SK_TILE + (4 * t - nb * SK_TILE);
+  }
   pdl_wait();
   float4* xr = reinterpret_cast<float4*>(x + (size_t)row * ldx);
   float4 v = on ? xr[t] : make_float4(0, 0, 0, 0);
-  for (int sp0 = 0; sp0 < splits; sp0 += 4) {
+  for (int sp0 = s0; sp0 < s1; sp0 += 4) {
     float4 pv[4];
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
-      const float4* pr = reinterpret_cast<const float4*>(partials + (size_t)(sp0 + u) * (size_t)split_stride + (size_t)row * D);
-      pv[u] = (sp0 + u < splits && on) ? __ldcg(pr + t) : make_float4(0, 0, 0, 0);
+      const float4* pr = reinterpret_cast<const float4*>(partials + (size_t)(sp0 + u) * (size_t)stride + (size_t)off);
+      pv[u] = (sp0 + u < s1 && on) ? __ldcg(pr) : make_float4(0, 0, 0, 0);
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u)          // fixed order: bitwise reproducible
-      if (sp0 + u < splits) { v.x += pv[u].x; v.y += pv[u].y; v.z += pv[u].z; v.w += pv[u].w; }
+      if (sp0 + u < s1) { v.x += pv[u].x; v.y += pv[u].y; v.z += pv[u].z; v.w += pv[u].w; }
   }
   float s = 0.f;
   if (on) { xr[t] = v; s = (v.x + v.y) + (v.z + v.w); }
@@ -642,34 +653,39 @@ extern "C" int vlfm_layernorm_x2(const float* d_x, const float* d_gamma, const f
   return layernorm_impl(d_x, d_gamma, d_beta, d_out_hi, d_out_lo, d_out32, rows, D, ldx, ldo16, ldo32, eps, stream);
 }
 
-static int layernorm_reduce_impl(float* d_x, const float* d_partials, int splits, long long split_stride, const float* d_gamma,
-                                 const float* d_beta, void* d_out16, void* d_out16_lo, float* d_out32, int rows, int D, int ldx, int ldo16, int ldo32,
-                                 float eps, void* stream) {
+namespace vlfm {
+int layernorm_reduce_impl(float* d_x, const float* d_partials, const SplitK& sk, const float* d_gamma,
+                          const float* d_beta, void* d_out16, void* d_out16_lo, float* d_out32, int rows, int D, int ldx, int ldo16, int ldo32,
+                          float eps, void* stream) {
   __half* lo16 = (__half*)d_out16_lo;
-  if (!d_x || !d_partials || !d_gamma || !d_beta || (!d_out16 && !d_out32) || rows < 1 || D < 1 || splits < 1 || splits > 16) {
+  if (!d_x || !d_partials || !d_gamma || !d_beta || (!d_out16 && !d_out32) || rows < 1 || D < 1 || sk.splits < 0 || sk.splits > 16 ||
+      (sk.splits == 0 && (sk.ctas < 1 || sk.row_tiles < 1 || sk.tiles != sk.row_tiles * ((D + SK_TILE - 1) / SK_TILE) || sk.num_k < 1))) {
     set_error("vlfm_layernorm_reduce: bad argument"); return VLFM_E_INVALID; }
-  if ((D & 3) || (ldx & 3) || (ldo16 & 3) || (ldo32 & 3) || (split_stride & 3)) { set_error("vlfm_layernorm_reduce: D and strides must be multiples of 4"); return VLFM_E_UNSUPPORTED; }
+  if ((D & 3) || (ldx & 3) || (ldo16 & 3) || (ldo32 & 3) || (sk.stride & 3)) { set_error("vlfm_layernorm_reduce: D and strides must be multiples of 4"); return VLFM_E_UNSUPPORTED; }
   cudaStream_t st = (cudaStream_t)stream;
   const dim3 grid(rows);
   __half* o16 = (__half*)d_out16;
   cudaError_t e;
   if (D > 1536) { set_error("vlfm_layernorm_reduce: D=%d too large (max 1536)", D); return VLFM_E_UNSUPPORTED; }
   const int threads = (((D >> 2) + 31) / 32) * 32;
-  e = launch_pdl(layernorm_reduce_kernel, grid, dim3(threads), 0, st, d_x, d_partials, splits, split_stride, d_gamma, d_beta, o16, d_out32, rows, D, ldx, ldo16, ldo32, eps, lo16);
+  e = launch_pdl(layernorm_reduce_kernel, grid, dim3(threads), 0, st, d_x, d_partials, sk, d_gamma, d_beta, o16, d_out32, rows, D, ldx, ldo16, ldo32, eps, lo16);
   { int rc = check_cuda(e, "layernorm_reduce_kernel"); if (rc) return rc; }
   count_launch();
   return VLFM_OK;
 }
+}  // namespace vlfm
 extern "C" int vlfm_layernorm_reduce(float* d_x, const float* d_partials, int splits, long long split_stride, const float* d_gamma,
                                      const float* d_beta, void* d_out16, float* d_out32, int rows, int D, int ldx, int ldo16, int ldo32,
                                      float eps, void* stream) {
-  return layernorm_reduce_impl(d_x, d_partials, splits, split_stride, d_gamma, d_beta, d_out16, nullptr, d_out32, rows, D, ldx, ldo16, ldo32, eps, stream);
+  if (splits < 1) { set_error("vlfm_layernorm_reduce: bad argument"); return VLFM_E_INVALID; }
+  return layernorm_reduce_impl(d_x, d_partials, SplitK{splits, split_stride}, d_gamma, d_beta, d_out16, nullptr, d_out32, rows, D, ldx, ldo16, ldo32, eps, stream);
 }
 extern "C" int vlfm_layernorm_reduce_x2(float* d_x, const float* d_partials, int splits, long long split_stride, const float* d_gamma,
                                         const float* d_beta, void* d_out_hi, void* d_out_lo, float* d_out32, int rows, int D, int ldx, int ldo16,
                                         int ldo32, float eps, void* stream) {
   if (!d_out_hi || !d_out_lo) { set_error("vlfm_layernorm_reduce_x2: null output"); return VLFM_E_INVALID; }
-  return layernorm_reduce_impl(d_x, d_partials, splits, split_stride, d_gamma, d_beta, d_out_hi, d_out_lo, d_out32, rows, D, ldx, ldo16, ldo32, eps, stream);
+  if (splits < 1) { set_error("vlfm_layernorm_reduce_x2: bad argument"); return VLFM_E_INVALID; }
+  return layernorm_reduce_impl(d_x, d_partials, SplitK{splits, split_stride}, d_gamma, d_beta, d_out_hi, d_out_lo, d_out32, rows, D, ldx, ldo16, ldo32, eps, stream);
 }
 
 extern "C" int vlfm_attention_f16(const void* d_q, const void* d_k, const void* d_v, void* d_o, int B, int heads, int Nq,
