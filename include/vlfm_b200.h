@@ -214,8 +214,12 @@ int vlfm_layernorm_reduce_x2(float* d_x, const float* d_partials, int splits, lo
 int vlfm_split_x2(const float* d_src, void* d_hi, void* d_lo, long long n, void* stream);
 int vlfm_attention_f32(const float* d_q, const float* d_k, const float* d_v, void* d_o_hi, void* d_o_lo, int B, int heads, int Nq,
                        int Nk, int hd, int ldq, int ldk, int ldv, int ldo, float scale, void* stream);
-/* ITC head (match_head="itc"): cos[b] = max_q <normalize(proj[b,q,:]), text>.  */
+/* ITC head (match_head="itc"): cos[b] = max_q <normalize(proj[b,q,:]), text>.
+ * vlfm_itc_head_multi: the same against P prompts, text [P, D] (rows L2-normalised) -> out[b * ldo + p]; one launch, the
+ * query norms computed once.  Column p is bitwise equal to vlfm_itc_head on text[p] (vlfm_itc_head is the P = 1 case).
+ * VLFM_E_INVALID for NULL pointers, B < 1, P < 1 or ldo < P. */
 int vlfm_itc_head(const float* d_proj, const float* d_text, float* d_out, int B, int Q, int D, void* stream);
+int vlfm_itc_head_multi(const float* d_proj, const float* d_text, float* d_out, int B, int P, int Q, int D, int ldo, void* stream);
 
 /* ----------------------------------------------- GroundingDINO Swin-T backbone ---- */
 /* Replaces the image branch of groundingdino's predict() up to the backbone feature maps

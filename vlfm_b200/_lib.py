@@ -90,6 +90,7 @@ _SIGNATURES = {
     "vlfm_holes_batch_workspace_bytes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "vlfm_fill_small_holes_batch": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_double, _P, _P, C.c_size_t, _P, _P, C.c_size_t, _P]),
     "vlfm_itc_head": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
+    "vlfm_itc_head_multi": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "vlfm_groupnorm_rows": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_float, _P, C.c_int, C.c_int, _P]),
     "vlfm_im2col3x3s2": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "vlfm_mask_rows_f16": (C.c_int, [_P, _P, _P, C.c_long, C.c_int, _P]),

@@ -447,26 +447,59 @@ attention_kernel(AttnArgs a) {
 }
 
 // -------------------------------------------------------------------- ITC head ----
-// proj [B, Q, D] fp32 (vision_proj output), text [D] fp32 L2-normalised -> cos [B]
-__global__ void itc_head_kernel(const float* __restrict__ proj, const float* __restrict__ text,
-                                float* __restrict__ out, int Q, int D) {
+// proj [B, Q, D] fp32 (vision_proj output), text [P, D] fp32 rows L2-normalised -> out[b * ldo + p] = max_q cos(proj[b,q], text[p]).
+// One CTA per image.  Warp w owns queries w, w + nw, ...; the prompts go in chunks of ITC_PT, each chunk reading a query row once.
+// The query norm is reduced in the first chunk and kept in shared memory (den[Q], dynamic) for the others.  Every (q, p) dot
+// product is the same lane-strided fp32 sum and xor-shuffle tree whatever P is, so column p equals a P = 1 launch on text[p].
+constexpr int ITC_PT = 8;
+
+__global__ void __launch_bounds__(256) itc_head_kernel(const float* __restrict__ proj, const float* __restrict__ text,
+                                                       float* __restrict__ out, int P, int Q, int D, int ldo) {
+  extern __shared__ float den[];
+  __shared__ float best[ITC_PT][32];
   const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  __shared__ float best[32];
-  float mx = -INFINITY;
-  for (int q = warp; q < Q; q += nw) {
-    const float* p = proj + ((size_t)b * Q + q) * D;
-    float nn = 0.f, dt = 0.f;
-    for (int d = lane; d < D; d += 32) { float v = p[d]; nn += v * v; dt += v * text[d]; }
+  for (int p0 = 0; p0 < P; p0 += ITC_PT) {
+    const int np = min(ITC_PT, P - p0);
+    const float* tx = text + (size_t)p0 * D;
+    float mx[ITC_PT];
 #pragma unroll
-    for (int o = 16; o; o >>= 1) { nn += __shfl_xor_sync(0xffffffffu, nn, o); dt += __shfl_xor_sync(0xffffffffu, dt, o); }
-    mx = fmaxf(mx, dt / fmaxf(sqrtf(nn), 1e-12f));   // F.normalize eps
-  }
-  if (lane == 0) best[warp] = mx;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float m = best[0];
-    for (int i = 1; i < nw; ++i) m = fmaxf(m, best[i]);
-    out[b] = m;
+    for (int j = 0; j < ITC_PT; ++j) mx[j] = -INFINITY;
+    for (int q = warp; q < Q; q += nw) {
+      const float* pr = proj + ((size_t)b * Q + q) * D;
+      float nn = 0.f, dt[ITC_PT];
+#pragma unroll
+      for (int j = 0; j < ITC_PT; ++j) dt[j] = 0.f;
+      for (int d = lane; d < D; d += 32) {
+        const float v = pr[d];
+        if (p0 == 0) nn += v * v;
+#pragma unroll
+        for (int j = 0; j < ITC_PT; ++j)
+          if (j < np) dt[j] += v * tx[(size_t)j * D + d];
+      }
+#pragma unroll
+      for (int o = 16; o; o >>= 1) {
+        if (p0 == 0) nn += __shfl_xor_sync(0xffffffffu, nn, o);
+#pragma unroll
+        for (int j = 0; j < ITC_PT; ++j)
+          if (j < np) dt[j] += __shfl_xor_sync(0xffffffffu, dt[j], o);
+      }
+      const float dq = p0 == 0 ? fmaxf(sqrtf(nn), 1e-12f) : den[q];   // F.normalize eps
+      // the owning warp writes den[q] here and reads it in later chunks; the CTA barrier closing each chunk orders the two
+      if (p0 == 0 && lane == 0) den[q] = dq;
+#pragma unroll
+      for (int j = 0; j < ITC_PT; ++j) mx[j] = fmaxf(mx[j], dt[j] / dq);
+    }
+    if (lane == 0) {
+#pragma unroll
+      for (int j = 0; j < ITC_PT; ++j) best[j][warp] = mx[j];
+    }
+    __syncthreads();
+    if (threadIdx.x < np) {
+      float m = best[threadIdx.x][0];
+      for (int i = 1; i < nw; ++i) m = fmaxf(m, best[threadIdx.x][i]);
+      out[(size_t)b * ldo + p0 + threadIdx.x] = m;
+    }
+    __syncthreads();
   }
 }
 
@@ -767,10 +800,17 @@ extern "C" int vlfm_split_x2(const float* d_src, void* d_hi, void* d_lo, long lo
   return VLFM_OK;
 }
 
-extern "C" int vlfm_itc_head(const float* d_proj, const float* d_text, float* d_out, int B, int Q, int D, void* stream) {
-  if (!d_proj || !d_text || !d_out || B < 1) { set_error("vlfm_itc_head: bad argument"); return VLFM_E_INVALID; }
-  itc_head_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(d_proj, d_text, d_out, Q, D);
+extern "C" int vlfm_itc_head_multi(const float* d_proj, const float* d_text, float* d_out, int B, int P, int Q, int D, int ldo,
+                                   void* stream) {
+  if (!d_proj || !d_text || !d_out || B < 1 || P < 1 || Q < 1 || D < 1 || ldo < P || (size_t)Q * sizeof(float) > 48 * 1024) {
+    set_error("vlfm_itc_head_multi: bad argument (B, P, Q, D >= 1, ldo >= P, Q <= 12288)"); return VLFM_E_INVALID; }
+  itc_head_kernel<<<B, 256, Q * sizeof(float), (cudaStream_t)stream>>>(d_proj, d_text, d_out, P, Q, D, ldo);
   VLFM_CHECK_LAUNCH("itc_head_kernel");
   count_launch();
   return VLFM_OK;
+}
+
+extern "C" int vlfm_itc_head(const float* d_proj, const float* d_text, float* d_out, int B, int Q, int D, void* stream) {
+  if (!d_proj || !d_text || !d_out || B < 1) { set_error("vlfm_itc_head: bad argument"); return VLFM_E_INVALID; }
+  return vlfm_itc_head_multi(d_proj, d_text, d_out, B, 1, Q, D, 1, stream);
 }

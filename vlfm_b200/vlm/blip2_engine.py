@@ -52,6 +52,10 @@ class Blip2ITCEngine:
         rows = min(max_batch * dims.tokens, 1024)      # larger problems never split K (2-CTA 256x256 tiles)
         self._partials = torch.empty(8 * rows * max(dims.v_hidden, dims.q_hidden), dtype=F32, device=self.dev)
         self._fold_layer0()
+        self._many_out: Dict[int, torch.Tensor] = {}   # forward_many / head outputs [max_batch, P], one per P
+        # bumped by every forward / forward_many / encode_text: q_proj holds the image features of the forward that set the
+        # current value, so a caller that recorded it can score that forward's images against new prompts with head() alone
+        self.generation = 0
 
     # ------------------------------------------------------------------ weights ----
     def _load(self, sd: Dict[str, torch.Tensor]) -> None:
@@ -384,6 +388,7 @@ class Blip2ITCEngine:
     def encode_text(self, token_ids: Sequence[int]) -> torch.Tensor:
         """Q-Former text branch (query_length=0) -> normalised text feature [proj]; run once per prompt."""
         d = self.d
+        self.generation += 1
         ids = torch.tensor(list(token_ids), dtype=torch.long, device=self.dev)
         S = len(ids)
         assert 1 <= S <= self.d.queries * self.max_batch and S <= 272
@@ -412,6 +417,7 @@ class Blip2ITCEngine:
         B, Hh, Ww, _ = images.shape
         assert B <= self.max_batch and images.dtype == torch.uint8 and images.is_contiguous()
         key = (B, Hh, Ww)
+        self.generation += 1
         with torch.cuda.device(self.dev):
             if not self.use_graph:
                 mid = torch.empty(B, Hh, self.d.image, 3, dtype=torch.uint8, device=self.dev)
@@ -431,6 +437,30 @@ class Blip2ITCEngine:
             static_in.copy_(images, non_blocking=True)
             g.replay()
         return self.out[:B]
+
+    @torch.inference_mode()
+    def forward_many(self, images: torch.Tensor, text_feats: torch.Tensor) -> torch.Tensor:
+        """images [B,H,W,3] uint8 on the device, text_feats [P, proj] fp32 normalised (encode_text rows) -> cosines [B, P]
+        (device, fp32): one image forward and one head launch for all P prompts.  Column p is bitwise equal to forward()
+        after set_text(text_feats[p]).  The result is a view of a buffer kept per P, rewritten by the next call."""
+        self.forward(images)
+        return self.head(text_feats, images.shape[0])
+
+    @torch.inference_mode()
+    def head(self, text_feats: torch.Tensor, B: int) -> torch.Tensor:
+        """Scores the image features the last forward left in q_proj (its first B images) against text_feats [P, proj]
+        -> [B, P] (device, fp32, same buffer as forward_many's).  Runs no forward."""
+        P = text_feats.shape[0]
+        assert 1 <= B <= self.max_batch and text_feats.shape == (P, self.d.proj) and text_feats.dtype == F32
+        assert text_feats.is_contiguous() and text_feats.is_cuda
+        out = self._many_out.get(P)
+        if out is None:
+            out = self._many_out[P] = torch.empty(self.max_batch, P, dtype=F32, device=self.dev)
+        with torch.cuda.device(self.dev):
+            rc = self.lib.vlfm_itc_head_multi(self.q_proj.data_ptr(), text_feats.data_ptr(), out.data_ptr(), B, P, self.d.queries,
+                                              self.d.proj, P, _lib.stream_ptr())
+        _lib.check(rc, "vlfm_itc_head_multi")
+        return out[:B]
 
     def launches_per_forward(self) -> int:
         d = self.d

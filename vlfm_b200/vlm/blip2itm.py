@@ -10,7 +10,7 @@ from __future__ import annotations
 import os
 import re
 import zlib
-from typing import Any, Dict, List, Optional, Sequence
+from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -134,36 +134,105 @@ class BLIP2ITM:
         self.tokenizer = tokenizer
         self.engine = Blip2ITCEngine(self.dims, state_dict, device=device, max_batch=max_batch)
         self._text_cache: Dict[str, torch.Tensor] = {}
+        self._stacks: Dict[Tuple[str, ...], torch.Tensor] = {}
         self._cur_text: Optional[str] = None
         self._pin: Optional[torch.Tensor] = None
         self._dev_img: Optional[torch.Tensor] = None
+        self._seen: Optional[torch.Tensor] = None
+        self._side: Optional[torch.cuda.Stream] = None
+        # the host frame of the last host-side forward: (caller's object, shape, dtype, engine generation, the bytes it saw)
+        self._frame: Optional[Tuple[np.ndarray, Tuple[int, ...], np.dtype, int, np.ndarray]] = None
+
+    def _text(self, txt: str) -> torch.Tensor:
+        if txt not in self._text_cache:
+            self._text_cache[txt] = self.engine.encode_text(self.tokenizer(pre_caption(txt)))
+        return self._text_cache[txt]
 
     def _use_text(self, txt: str) -> None:
         if txt != self._cur_text:
-            if txt not in self._text_cache:
-                self._text_cache[txt] = self.engine.encode_text(self.tokenizer(pre_caption(txt)))
-            self.engine.set_text(self._text_cache[txt])
+            self.engine.set_text(self._text(txt))
             self._cur_text = txt
+
+    def _text_stack(self, prompts: Sequence[str]) -> torch.Tensor:
+        """[P, proj] text features of ``prompts``, stacked once per prompt tuple."""
+        key = tuple(prompts)
+        if not key:
+            raise ValueError("BLIP2ITM: at least one prompt is needed")
+        if key not in self._stacks:
+            self._stacks[key] = torch.stack([self._text(p) for p in key])
+        return self._stacks[key]
 
     def cosine_device(self, images: torch.Tensor, txt: str) -> torch.Tensor:
         """images [B,H,W,3] uint8 already in HBM -> cosines [B] (device)."""
         self._use_text(txt)
         return self.engine.forward(images)
 
-    def cosine(self, image: np.ndarray, txt: str) -> float:
-        """blip2itm.py:37-54: host uint8 RGB frame + prompt -> Python float."""
-        self._use_text(txt)
+    def cosine_device_many(self, images: torch.Tensor, prompts: Sequence[str]) -> torch.Tensor:
+        """images [B,H,W,3] uint8 already in HBM -> cosines [B, P] (device, fp32) against every prompt, from one forward.
+        Feeds ``ValueMapBatch.update(values.double(), ...)`` directly.  The result is rewritten by the next call."""
+        return self.engine.forward_many(images, self._text_stack(prompts))
+
+    def _cached(self, image: Any) -> bool:
+        """True when the engine still holds the image features of ``image``: the same object as the last host-side
+        forward's frame, same shape and dtype, the same bytes (callers may refill one buffer in place) and no forward since."""
+        f = self._frame
+        if f is None or image is not f[0] or image.shape != f[1] or image.dtype != f[2] or self.engine.generation != f[3]:
+            return False
+        a, b = np.ascontiguousarray(image, dtype=np.uint8), f[4]
+        if a.nbytes % 8 == 0:        # compare 8 bytes at a time
+            a, b = a.reshape(-1).view(np.uint64), b.reshape(-1).view(np.uint64)
+        return bool(np.array_equal(a, b))
+
+    def _forward_host(self, image: Any, run) -> torch.Tensor:
+        """One H2D of a host frame, then ``run(device frame)`` enqueued; records the frame for ``_cached``."""
+        arg, self._frame = image, None
         image = np.ascontiguousarray(image, dtype=np.uint8)
         if self._pin is None or self._pin.shape[1:] != image.shape:
             self._pin = torch.empty((1,) + image.shape, dtype=torch.uint8).pin_memory()
             self._dev_img = torch.empty((1,) + image.shape, dtype=torch.uint8, device=self.device)
         src = torch.from_numpy(image)
-        if src.is_pinned():          # caller's frame already lives in page-locked memory: DMA straight from it (the call syncs below)
+        if src.is_pinned():          # caller's frame already lives in page-locked memory: DMA straight from it (the call syncs after)
             self._dev_img.copy_(src[None], non_blocking=True)
+            # keep the bytes this forward sees: a D2H of the uploaded frame on a side stream runs on the copy engine beside the
+            # forward.  A host-side np.copyto here cost ~5 % of the batch-1 host step on an H100 80GB HBM3 (700 W); the DMA
+            # cost nothing measurable.
+            if self._seen is None or self._seen.shape[1:] != image.shape:
+                self._seen = torch.empty((1,) + image.shape, dtype=torch.uint8).pin_memory()
+                self._side = torch.cuda.Stream(self.device)
+            main = torch.cuda.current_stream(self.device)
+            self._side.wait_stream(main)
+            with torch.cuda.stream(self._side):
+                self._seen.copy_(self._dev_img, non_blocking=True)
+            out = run(self._dev_img)
+            main.wait_stream(self._side)    # the caller's sync after this call covers the snapshot too
+            seen = self._seen[0].numpy()
         else:
             self._pin[0].numpy()[...] = image
             self._dev_img.copy_(self._pin, non_blocking=True)
-        return float(self.engine.forward(self._dev_img)[0].item())  # .item(): D2H sync, as in the reference
+            out = run(self._dev_img)
+            seen = self._pin[0].numpy()
+        self._frame = (arg, arg.shape, arg.dtype, self.engine.generation, seen) if isinstance(arg, np.ndarray) else None
+        return out
+
+    def cosine(self, image: np.ndarray, txt: str) -> float:
+        """blip2itm.py:37-54: host uint8 RGB frame + prompt -> Python float.  When ``image`` is the frame of the last
+        host-side forward (same object, unchanged bytes, no forward since), only the ITC head runs: a policy scoring one
+        frame against several prompts pays for one image forward.  Pass a different object to force a forward."""
+        feat = self._text(txt)
+        if self._cached(image):
+            return float(self.engine.head(feat[None], 1)[0, 0].item())
+        self._use_text(txt)
+        return float(self._forward_host(image, self.engine.forward)[0].item())  # .item(): D2H sync, as in the reference
+
+    def cosine_many(self, image: np.ndarray, prompts: Sequence[str]) -> List[float]:
+        """Host uint8 RGB frame + P prompts -> P cosines: one H2D, one forward (none when the frame is cached, as in
+        ``cosine``), one head launch and one D2H.  Element p is bitwise equal to ``cosine(image, prompts[p])``."""
+        feats = self._text_stack(prompts)
+        if self._cached(image):
+            out = self.engine.head(feats, 1)
+        else:
+            out = self._forward_host(image, lambda dev: self.engine.forward_many(dev, feats))
+        return out[0].tolist()
 
 
 _SHARED: Dict[str, BLIP2ITM] = {}
@@ -182,3 +251,6 @@ class BLIP2ITMClient:
 
     def cosine(self, image: np.ndarray, txt: str) -> float:
         return self.model.cosine(image, txt)
+
+    def cosine_many(self, image: np.ndarray, prompts: Sequence[str]) -> List[float]:
+        return self.model.cosine_many(image, prompts)
