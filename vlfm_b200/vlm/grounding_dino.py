@@ -137,6 +137,7 @@ class GroundingDINO:
         self.tokenizer = tokenizer
         self._pin: Optional[torch.Tensor] = None
         self._dev: Optional[torch.Tensor] = None
+        self._pin_ev: Optional[torch.cuda.Event] = None
         self._static: Dict[Any, Dict[str, Any]] = {}
         self._graph_ok = os.environ.get("VLFM_GDINO_GRAPH", "1") != "0"
         self._graph_max_batch = int(os.environ.get("VLFM_GDINO_GRAPH_MAX_BATCH", "4"))
@@ -201,11 +202,17 @@ class GroundingDINO:
     def raw_outputs(self, image: np.ndarray, input_ids: List[int]):
         """-> (sigmoid logits [900,256], boxes [900,4] cxcywh) on the device."""
         image = np.ascontiguousarray(image, dtype=np.uint8)
+        if self._pin_ev is not None:
+            # the last call's copy out of the page-locked buffer is asynchronous: overwriting the buffer before it has executed
+            # would hand that call this call's frame
+            self._pin_ev.synchronize()
         if self._pin is None or self._pin.shape[1:] != image.shape:
             self._pin = torch.empty((1,) + image.shape, dtype=torch.uint8).pin_memory()
             self._dev = torch.empty((1,) + image.shape, dtype=torch.uint8, device=self.device)
         self._pin[0].numpy()[...] = image
         self._dev.copy_(self._pin, non_blocking=True)
+        self._pin_ev = torch.cuda.Event()
+        self._pin_ev.record()
         logits, boxes = self.raw_outputs_device(self._dev, input_ids)
         return logits[0], boxes[0]
 
