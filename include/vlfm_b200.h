@@ -156,8 +156,9 @@ int vlfm_fill_small_holes(const float* d_depth, int H, int W, double area_thresh
  * partial sums in d_partials (no atomics) and the LayerNorm launch adds them to x in K order before normalising.  Below one
  * wave of 128 x 128 tiles the split is stream-K over one CTA per SM: (SMs + tiles - 1) slabs of 130 x 128 floats (66.5 KB);
  * a smaller d_partials lowers the CTA count, and below tiles + 1 CTAs the GEMM runs unsplit.  Above one wave the splits are
- * uniform (>= splits * M * N floats, splits <= 8); without d_partials (or when it is too small) they fall back to
- * red.global.add into x.  Stream-K results depend on the SM count: bitwise reproducible across cards with the same count.
+ * uniform (>= splits * M * N floats, splits <= 8); without d_partials (or when it is too small) they run unsplit: this
+ * call never reduces with red.global.add (only vlfm_gemm_f16 with VLFM_EPI_BIAS_RESID_F32 does).  Stream-K results depend on
+ * the SM count: bitwise reproducible across cards with the same count.
  * Replaces `x = x + proj(...)` followed by `layer_norm` in the BLIP-2 forward (blip2itm.py:52 through lavis).            */
 int vlfm_gemm_f16_resid_ln(const void* d_A, const void* d_W, const float* d_bias, float* d_x, int M, int N, int K,
                            int lda, int ldw, int ldx, const float* d_gamma, const float* d_beta, void* d_out16, int ld16,

@@ -88,20 +88,32 @@ def test_gemm_x2_resid_layernorm(M, N, K):
         assert all(torch.equal(p, q) for p, q in zip(o, outs[0]))
 
 
-@pytest.mark.parametrize("B,heads,Nq,Nk,hd", [(1, 12, 32, 32, 64), (1, 12, 32, 257, 64), (3, 12, 32, 257, 64), (1, 2, 9, 9, 32), (2, 2, 8, 17, 32)])
+# 12 heads x 64 at 32 queries: the row-group count z of vlfm_attention_f32 is 4 up to B = 5, 3 at B = 6 (passes of 24 rows: the
+# second one is partial), 2 at B = 8 and 1 from B = 12 (each warp loops over four query rows)
+@pytest.mark.parametrize("B,heads,Nq,Nk,hd", [(1, 12, 32, 32, 64), (1, 12, 32, 257, 64), (3, 12, 32, 257, 64), (1, 2, 9, 9, 32), (2, 2, 8, 17, 32),
+                                               (6, 12, 32, 257, 64), (8, 12, 32, 257, 64), (12, 12, 32, 257, 64), (32, 12, 32, 257, 64),
+                                               (2, 12, 32, 1, 64), (2, 12, 32, 272, 64), (3, 12, 1, 257, 64), (3, 12, 33, 257, 64)])
 def test_attention_f32_vs_float64(B, heads, Nq, Nk, hd):
+    """The engine's strides: q a column slice of the [B*Nq, 3*H] q/k/v buffer, K / V one layer's slices of the cross-attention
+    buffer [B*Nk, 6*2*H] (all layers' K|V side by side); hi / lo NaN-filled with 8 spare rows and columns that must stay NaN."""
     L, lib = _lib()
-    g = torch.Generator(device="cpu").manual_seed(Nq * 3 + Nk)
+    g = torch.Generator(device="cpu").manual_seed(Nq * 3 + Nk + 1000 * B)
     H = heads * hd
-    q, k, v = (torch.randn(B * n, H, generator=g).cuda() for n in (Nq, Nk, Nk))
-    hi, lo = torch.empty(B * Nq, H, dtype=torch.float16, device="cuda"), torch.empty(B * Nq, H, dtype=torch.float16, device="cuda")
+    qbuf = torch.randn(B * Nq, 3 * H, generator=g).cuda()
+    kvbuf = torch.randn(B * Nk, 6 * 2 * H, generator=g).cuda()
+    j = B % 6
+    q, k, v = qbuf[:, :H], kvbuf[:, 2 * j * H : (2 * j + 1) * H], kvbuf[:, (2 * j + 1) * H : (2 * j + 2) * H]
+    hi, lo = (torch.full((B * Nq + 8, H + 8), float("nan"), dtype=torch.float16, device="cuda") for _ in range(2))
     sc = hd ** -0.5
-    L.check(lib.vlfm_attention_f32(q.data_ptr(), k.data_ptr(), v.data_ptr(), hi.data_ptr(), lo.data_ptr(), B, heads, Nq, Nk, hd, H, H, H, H,
-                                   ctypes.c_float(sc), L.stream_ptr()), "attention f32")
+    L.check(lib.vlfm_attention_f32(q.data_ptr(), k.data_ptr(), v.data_ptr(), hi.data_ptr(), lo.data_ptr(), B, heads, Nq, Nk, hd, q.stride(0),
+                                   k.stride(0), v.stride(0), hi.stride(0), ctypes.c_float(sc), L.stream_ptr()), "attention f32")
     torch.cuda.synchronize()
-    qd, kd, vd = (t.double().view(B, -1, heads, hd).transpose(1, 2) for t in (q, k, v))
+    for t in (hi, lo):
+        assert bool(torch.isnan(t[B * Nq :]).all()) and bool(torch.isnan(t[:, H:]).all()), "spare rows / columns were written"
+        assert bool(torch.isfinite(t[: B * Nq, :H]).all()), "output rows left unwritten or non-finite"
+    qd, kd, vd = (t.double().reshape(B, -1, heads, hd).transpose(1, 2) for t in (q, k, v))
     ref = (torch.softmax(qd @ kd.transpose(-1, -2) * sc, -1) @ vd).transpose(1, 2).reshape(B * Nq, H)
-    got = hi.double() + lo.double() / 2048.0
+    got = hi[: B * Nq, :H].double() + lo[: B * Nq, :H].double() / 2048.0
     assert float((got - ref).abs().max()) <= 2e-6 * max(1.0, float(ref.abs().max()))
 
 

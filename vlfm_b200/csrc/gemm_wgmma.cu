@@ -675,6 +675,13 @@ static int gemm_dispatch(const void* d_A, const void* d_W, int M, int N, int K, 
   const char* force = getenv("VLFM_GEMM_FORCE");   // development sweep: "bn:splits" (grid launches only)
   const bool resid = epilogue == VLFM_EPI_BIAS_RESID_F32;
   const int tiles128 = rt * ((N + BM - 1) / BM);
+  // A resid-LN call (layout != null) never reduces with red.global.add: its splits must fit the workspace as partial sums, so a
+  // split that does not fit runs unsplit.  Only vlfm_gemm_f16 with the residual epilogue (no workspace) splits into x atomically.
+  long long split_cap = num_k;
+  if (layout) {
+    split_cap = (long long)(partial_bytes / ((size_t)M * (size_t)N * 4));
+    if (split_cap < 1) split_cap = 1;
+  }
   int best_bn = 128, best_s = 1;
   bool best_tail = tail;
   if (tiles128 < sms && resid && d_partials && !force) {
@@ -704,9 +711,9 @@ static int gemm_dispatch(const void* d_A, const void* d_W, int M, int N, int K, 
     }
   } else {
     // Tile / split-K plan from a small cost model (us): waves x (fixed + bytes a CTA must pull / its share of the L2->SM
-    // bandwidth).  Never spill into a second wave for a handful of CTAs; split K only for the fp32 residual epilogue (red.add,
-    // or without a workspace above it partial sums the LayerNorm launch reduces), and not at all for residual calls with a
-    // workspace below a wave (those are stream-K, or unsplit when the workspace is too small).
+    // bandwidth).  Never spill into a second wave for a handful of CTAs; split K only for the fp32 residual epilogue (partial
+    // sums the LayerNorm launch reduces, at most split_cap of them; red.add only for vlfm_gemm_f16 without a workspace), and not
+    // at all for residual calls with a workspace below a wave (those are stream-K, or unsplit when the workspace is too small).
     double best_t = 1e30;
     // Cost model:  t = waves * (c0 + K-blocks per CTA * per_kb),  per_kb = max(pipeline floor, CTAs * KB per K-block / chip L2->SM rate),
     //   c0 = prologue + epilogue per tile width, + split-K stores, + the tail-row work.  One CTA per SM (H100: 132).  The rate
@@ -720,6 +727,7 @@ static int gemm_dispatch(const void* d_A, const void* d_W, int M, int N, int K, 
         int smax = resid && !(d_partials && tiles128 < sms) ? num_k / 4 : 1;
         if (smax < 1) smax = 1;
         if (smax > 8) smax = 8;
+        if (smax > split_cap) smax = (int)split_cap;
         for (int sp = 1; sp <= smax; ++sp) {
           const double ctas = (double)mte * nt * sp;
           const int kb = (num_k + sp - 1) / sp;
@@ -741,6 +749,7 @@ static int gemm_dispatch(const void* d_A, const void* d_W, int M, int N, int K, 
     if (sscanf(force, "%d:%d", &fb, &fs) == 2 && (fb == 128 || fb == 96 || fb == 64 || fb == 32) && fs >= 1) {
       best_bn = fb;
       best_s = resid ? (fs > num_k ? num_k : fs) : 1;
+      if (best_s > split_cap) best_s = (int)split_cap;
     }
   }
   g.kb_per_split = (num_k + best_s - 1) / best_s;

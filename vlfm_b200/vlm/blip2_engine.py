@@ -25,6 +25,16 @@ from .preprocess import CLIP_MEAN, CLIP_STD, bicubic_tables
 F16, F32 = torch.float16, torch.float32
 
 
+def partials_floats(dims: Blip2Dims, max_batch: int) -> int:
+    """Size (floats) of the split-K workspace of the residual GEMM + LayerNorm calls: eight slabs of the residual stream for at
+    most 1024 rows (every stream-K plan, below one wave of tiles, and the uniform splits of the smaller batches), and at least
+    three for the whole batch: above one wave the GEMM plan splits the ViT's fc2 (K = 6144) two or three ways at some batches
+    (at B = 32: two), which is faster there than unsplit.  A split that does not fit runs unsplit (vlfm_gemm_f16_resid_ln never
+    reduces with atomics), so this size trades memory (139 MB at max_batch 32) for speed, not correctness."""
+    rows = max_batch * dims.tokens
+    return max(8 * min(rows, 1024), 3 * rows) * max(dims.v_hidden, dims.q_hidden)
+
+
 class Blip2ITCEngine:
     def __init__(self, dims: Blip2Dims, state_dict: Dict[str, torch.Tensor], device="cuda", max_batch: int = 1,
                  use_graph: bool = True) -> None:
@@ -49,8 +59,7 @@ class Blip2ITCEngine:
         # to the residual stream in split order by the LayerNorm launch): the cosine is bitwise reproducible run to run.
         # VLFM_DET_SPLITK=0 restores round 1's red.global.add reduction (order of arrival, ~6e-5 spread on the cosine).
         self.fuse_ln = os.environ.get("VLFM_DET_SPLITK", "1") != "0"
-        rows = min(max_batch * dims.tokens, 1024)      # larger problems never split K (2-CTA 256x256 tiles)
-        self._partials = torch.empty(8 * rows * max(dims.v_hidden, dims.q_hidden), dtype=F32, device=self.dev)
+        self._partials = torch.empty(partials_floats(dims, max_batch), dtype=F32, device=self.dev)
         self._fold_layer0()
         self._many_out: Dict[int, torch.Tensor] = {}   # forward_many / head outputs [max_batch, P], one per P
         # bumped by every forward / forward_many / encode_text: q_proj holds the image features of the forward that set the
