@@ -365,6 +365,39 @@ int vlfm_dbscan_largest_cluster(const double* d_points, const int32_t* d_gather,
                                 double* d_gathered, double* d_out, int32_t* d_out_count, void* d_workspace,
                                 size_t workspace_bytes, void* stream);
 
+/* --------------------------------------------------------------- map frames ---- */
+/* ValueMap.visualize / ObstacleMap.visualize (vlfm/mapping/value_map.py:189-219, obstacle_map.py:171-193) and the trajectory /
+ * marker overlay (vlfm/mapping/traj_visualizer.py) for a batch of environments.  Frames d_out / d_frames are
+ * [batch, G, G, 3] uint8 BGR, C-contiguous.  Bad arguments return VLFM_E_INVALID and launch nothing.
+ *
+ * vlfm_render_value: d_reduced [batch, G, G] float32 (reduced_f64 = 0) or float64 (1), call order; d_explored [nslots, G, G]
+ * uint8 or NULL, row i reads slot d_slots[i] (or i when d_slots is NULL); d_lut [256, 3] uint8 (cv2 COLORMAP_INFERNO).
+ * Cells with explored == 0 are zeroed, the map is flipped vertically, zero cells are white and the others take
+ * lut[uint8(((v - lo) / (hi - lo)) * 255)] computed in the map's dtype with one rounding per operation (lo / hi: min / max
+ * after the zero cells are set to the max; index 0 when hi == lo).  Two launches. */
+int vlfm_render_workspace_bytes(int batch, size_t* bytes);
+int vlfm_render_value(int G, int batch, const int32_t* d_slots, const void* d_reduced, int reduced_f64, const uint8_t* d_explored,
+                      const uint8_t* d_lut, uint8_t* d_out, void* d_workspace, size_t workspace_bytes, void* stream);
+/* vlfm_render_obstacle: obstacle / navigable / explored grids [nslots, G, G] uint8, frontier midpoints [nslots, max_frontiers, 2]
+ * float64 (x = col, y = row) and counts [nslots] int32 as ObstacleMapBatch holds them (row i reads slot d_slots[i]).  White,
+ * explored (200, 255, 200), nav == 0 the padding colour, obstacles black, frontier circles (radius 5, thickness 2,
+ * (200, 0, 0)) at int() of each midpoint, then flipped vertically.  Two launches. */
+int vlfm_render_obstacle(int G, int batch, const int32_t* d_slots, const uint8_t* d_obst, const uint8_t* d_nav, const uint8_t* d_explored,
+                         const double* d_frontiers, const int32_t* d_count, int max_frontiers, int pad_b, int pad_g, int pad_r,
+                         uint8_t* d_out, void* stream);
+/* vlfm_render_draw: draws each environment's ordered list of primitives onto its frame, with the pixels of
+ * cv2.line / cv2.circle (LINE_8, shift 0), clipping included.  h_lists (host, page-locked for an asynchronous upload) =
+ * offsets [batch + 1] (offsets[0] = 0, non-decreasing) followed by offsets[batch] records of VLFM_DRAW_RECORD_INTS int32:
+ *   {VLFM_DRAW_LINE,   x0, y0, x1, y1, 0,      thickness 1..16,         B | G << 8 | R << 16}
+ *   {VLFM_DRAW_CIRCLE, cx, cy, 0,  0,  radius 0..255, thickness -1 (filled) or 1..16, colour}
+ * with |coordinates| < 2^24.  list_ints = batch + 1 + 8 * offsets[batch]; the list is copied to d_lists (>= list_ints ints)
+ * with one cudaMemcpyAsync on `stream`, so h_lists must not be reused before that copy has executed.  One launch. */
+#define VLFM_DRAW_LINE 0
+#define VLFM_DRAW_CIRCLE 1
+#define VLFM_DRAW_RECORD_INTS 8
+int vlfm_render_draw(int G, int batch, uint8_t* d_frames, const int32_t* h_lists, size_t list_ints, int32_t* d_lists,
+                     size_t d_list_ints, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

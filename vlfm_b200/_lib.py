@@ -17,6 +17,7 @@ ST_FRONTIER_OVERFLOW = 4
 FUSE_WEIGHTED, FUSE_MAX_CONFIDENCE, FUSE_REPLACE, FUSE_EQUAL = 0, 1, 2, 4
 EPI_BIAS_F16, EPI_BIAS_GELU_F16, EPI_BIAS_RESID_F32, EPI_BIAS_F32, EPI_BIAS_RELU_F16 = 0, 1, 2, 3, 4
 EPI_BIAS_GELU_F16X2 = 6
+DRAW_LINE, DRAW_CIRCLE, DRAW_RECORD_INTS = 0, 1, 8
 
 
 class ValueParams(C.Structure):
@@ -104,6 +105,10 @@ _SIGNATURES = {
                                             C.c_size_t, _P]),
     "vlfm_dbscan_workspace_bytes": (C.c_int, [C.c_int, C.POINTER(C.c_size_t)]),
     "vlfm_dbscan_largest_cluster": (C.c_int, [_P, _P, C.c_int, C.c_double, C.c_int, _P, _P, _P, _P, C.c_size_t, _P]),
+    "vlfm_render_workspace_bytes": (C.c_int, [C.c_int, C.POINTER(C.c_size_t)]),
+    "vlfm_render_value": (C.c_int, [C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P, C.c_size_t, _P]),
+    "vlfm_render_obstacle": (C.c_int, [C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "vlfm_render_draw": (C.c_int, [C.c_int, C.c_int, _P, _P, C.c_size_t, _P, C.c_size_t, _P]),
 }
 
 _lib = None

@@ -27,7 +27,8 @@
 //   sector_edges     cv2.ellipse filled sector: 16.16 polygon from the host (integer-degree ellipse2Poly), same
 //                    scan conversion with fractional columns, PolyEdges from clipped end points at the grid edge.
 //   rays / thick     occlusion rays: cv2.polylines thickness 2 = FillConvexPoly rectangle (Line2 outline + two-edge
-//                    scan) + radius-1 discs, clipped like cv2 (grid + 2 px for the centre line, grid for Line2).
+//                    scan) + radius-1 discs, clipped like cv2 (grid + 2 px for the centre line, grid for Line2);
+//                    the rasteriser is csrc/cv_raster.cuh, shared with the map frames (csrc/render.cu).
 //   frontier_kernel  contour split at cells whose 3x3 blurred unexplored mask is 0, arc-length midpoints.
 #include <math.h>
 #include <string.h>
@@ -35,6 +36,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "cv_raster.cuh"
 
 namespace vlfm {
 
@@ -481,29 +483,7 @@ __global__ void zero_planes_plain_kernel(uint32_t* tog, uint32_t* orb, int words
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < words; i += gridDim.x * blockDim.x) { tog[i] = 0; orb[i] = 0; }
 }
 
-// cv::clipLine(Size2l(W, H), pt1, pt2) (oracle/cv_prims.py::clip_line): Cohen-Sutherland, intersections in double, truncated
-// toward zero.  cv2 clips every line to the image before walking it, so a line that leaves the grid is the walk of the CLIPPED
-// segment.  The end points are modified even when the function returns false (as in OpenCV).
-__device__ __forceinline__ long long clip_isect(long long a, long long b, long long c) {   // (int64)((double)a * b / c)
-  return (long long)__ddiv_rn(__dmul_rn((double)a, (double)b), (double)c);
-}
-__device__ bool clip_line(long long W, long long H, long long& x1, long long& y1, long long& x2, long long& y2) {
-  const long long right = W - 1, bottom = H - 1;
-  if (W <= 0 || H <= 0) return false;
-  int c1 = (x1 < 0) + (x1 > right) * 2 + (y1 < 0) * 4 + (y1 > bottom) * 8;
-  int c2 = (x2 < 0) + (x2 > right) * 2 + (y2 < 0) * 4 + (y2 > bottom) * 8;
-  if ((c1 & c2) == 0 && (c1 | c2) != 0) {
-    long long a;
-    if (c1 & 12) { a = c1 < 8 ? 0 : bottom; x1 += clip_isect(a - y1, x2 - x1, y2 - y1); y1 = a; c1 = (x1 < 0) + (x1 > right) * 2; }
-    if (c2 & 12) { a = c2 < 8 ? 0 : bottom; x2 += clip_isect(a - y2, x2 - x1, y2 - y1); y2 = a; c2 = (x2 < 0) + (x2 > right) * 2; }
-    if ((c1 & c2) == 0 && (c1 | c2) != 0) {
-      if (c1) { a = c1 == 1 ? 0 : right; y1 += clip_isect(a - x1, y2 - y1, x2 - x1); x1 = a; c1 = 0; }
-      if (c2) { a = c2 == 1 ? 0 : right; y2 += clip_isect(a - x2, y2 - y1, x2 - x1); x2 = a; c2 = 0; }
-    }
-  }
-  return (c1 | c2) == 0;
-}
-
+using cvr::clip_line;   // cv::clipLine (csrc/cv_raster.cuh)
 
 // cv2.ellipse filled sector: polygon (x, y in 16.16, last vertex = centre) from the host; CollectPolyEdges +
 // FillEdgeCollection (oracle/cv_draw.py::fill_poly_fixed / poly_edge).  One block; the image is the GW x GH grid, of which the
@@ -668,121 +648,25 @@ __global__ void rays_kernel(const ExEnv* __restrict__ envs) {
   }
 }
 
-// cv2 thickness-2 line into the byte image `cut` (oracle/cv_draw.py::thick_line2).  All geometry is in GRID coordinates (the
-// clipping rules refer to the grid); `cut` is the window at (ox, oy), pixels outside it are skipped.
-struct CutWin { uint8_t* img; int W, H, ox, oy; };
-__device__ __forceinline__ void put_px(const CutWin& c, long long x, long long y) {
-  x -= c.ox; y -= c.oy;
-  if (x >= 0 && x < c.W && y >= 0 && y < c.H) c.img[y * c.W + x] = 1;
-}
-__device__ __forceinline__ long long cdiv(long long a, long long b) {   // C truncating division (b > 0)
-  return a / b;
-}
-// drawing.cpp Line2: clipLine against the image scaled to 16.16, then a DDA between the clipped end points.  One WARP per line:
-// step i of the DDA is closed-form (x1 + i, y1 + i * y_step), lanes stride over the steps.
-__device__ void line2_fixed(const CutWin& c, int G, long long x1, long long y1, long long x2, long long y2, int lane) {
-  if (!clip_line((long long)G << XYS, (long long)G << XYS, x1, y1, x2, y2)) return;
-  long long dx = x2 - x1, dy = y2 - y1;
-  const long long ax = dx < 0 ? -dx : dx, ay = dy < 0 ? -dy : dy;
-  long long x_step, y_step, ecount;
-  if (ax > ay) {
-    if (dx < 0) { long long t = x1; x1 = x2; x2 = t; t = y1; y1 = y2; y2 = t; dy = -dy; }
-    x_step = XYONE; y_step = cdiv(dy << XYS, ax | 1); ecount = (x2 - x1) >> XYS;
-  } else {
-    if (dy < 0) { long long t = x1; x1 = x2; x2 = t; t = y1; y1 = y2; y2 = t; dx = -dx; }
-    x_step = cdiv(dx << XYS, ay | 1); y_step = XYONE; ecount = (y2 - y1) >> XYS;
+// cv2 thickness-2 line into the byte image `cut` (oracle/cv_draw.py::thick_line2) with the shared rasteriser (csrc/cv_raster.cuh).
+// All geometry is in GRID coordinates (the clipping rules refer to the grid); `cut` is the window at (ox, oy), pixels outside
+// it are skipped.
+struct CutWin {
+  uint8_t* img; int W, H, ox, oy;
+  __device__ __forceinline__ void put(long long x, long long y) const {
+    x -= ox; y -= oy;
+    if (x >= 0 && x < W && y >= 0 && y < H) img[y * W + x] = 1;
   }
-  x1 += XYONE >> 1; y1 += XYONE >> 1;
-  if (lane == 0) put_px(c, (x2 + (XYONE >> 1)) >> XYS, (y2 + (XYONE >> 1)) >> XYS);
-  if (ax > ay) {
-    const long long x = x1 >> XYS;
-    for (long long i = lane; i <= ecount; i += 32) put_px(c, x + i, (y1 + i * y_step) >> XYS);
-  } else {
-    const long long y = y1 >> XYS;
-    for (long long i = lane; i <= ecount; i += 32) put_px(c, (x1 + i * x_step) >> XYS, y + i);
+  __device__ __forceinline__ void span(long long y, long long x1, long long x2, int first, int step) const {
+    const long long wy = y - oy;
+    if (wy < 0 || wy >= H) return;
+    x1 -= ox; x2 -= ox;
+    for (long long x = (x1 < 0 ? 0 : x1) + first; x <= x2 && x < W; x += step) img[wy * W + x] = 1;
   }
-}
-__device__ __forceinline__ long long pick4(const long long (&a)[4], int i) { return i == 0 ? a[0] : (i == 1 ? a[1] : (i == 2 ? a[2] : a[3])); }
-
-// One warp per ray.  The two-edge scan of FillConvexPoly is replayed by every lane WITHOUT drawing, jumping from edge switch to
-// edge switch (<= 4 of them); between two switches both edge x positions are linear in the row, so the rows of such a span are
-// filled by the lanes in parallel.
+};
+// One warp per ray (r: end points in window coordinates)
 __device__ void thick_ray(const int4 r, uint8_t* __restrict__ cut, int W, int H, int ox, int oy, int G, int lane) {
-  const CutWin cw{cut, W, H, ox, oy};
-  // ThickLine (cv2 4.13): the integer centre line is first clipped to the image grown by the thickness on every side
-  long long px0 = r.x + ox + 2, py0 = r.y + oy + 2, px1 = r.z + ox + 2, py1 = r.w + oy + 2;
-  if (!clip_line((long long)G + 4, (long long)G + 4, px0, py0, px1, py1)) return;
-  px0 -= 2; py0 -= 2; px1 -= 2; py1 -= 2;
-  const long long x0 = px0 << XYS, y0 = py0 << XYS, x1 = px1 << XYS, y1 = py1 << XYS;
-  const double dx = (double)(x0 - x1) / 65536.0, dy = (double)(y1 - y0) / 65536.0;
-  double rr = dx * dx + dy * dy;
-  if (fabs(rr) > 2.220446049250313e-16) {
-    rr = 65536.0 / sqrt(rr);                                      // thickness 2 -> half width one pixel (16.16)
-    const long long dpx = (long long)rint(dy * rr), dpy = (long long)rint(dx * rr);
-    long long vx[4] = {x0 + dpx, x0 - dpx, x1 - dpx, x1 + dpx}, vy[4] = {y0 + dpy, y0 - dpy, y1 - dpy, y1 + dpy};
-    // FillConvexPoly (shift = 16): Line2 outline ...
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { const int j = (i + 3) & 3; line2_fixed(cw, G, vx[j], vy[j], vx[i], vy[i], lane); }
-    // ... + two-edge scan
-    const long long delta = XYONE >> 1;
-    int imin = 0;
-    long long ymin_f = vy[0], ymax_f = vy[0], xmin_f = vx[0], xmax_f = vx[0];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      if (vy[i] < ymin_f) { ymin_f = vy[i]; imin = i; }
-      ymax_f = vy[i] > ymax_f ? vy[i] : ymax_f; xmax_f = vx[i] > xmax_f ? vx[i] : xmax_f; xmin_f = vx[i] < xmin_f ? vx[i] : xmin_f;
-    }
-    long long ymin = (ymin_f + delta) >> XYS, ymax = (ymax_f + delta) >> XYS;
-    const long long xmin = (xmin_f + delta) >> XYS, xmax = (xmax_f + delta) >> XYS;
-    if (!(xmax < 0 || ymax < 0 || xmin >= G || ymin >= G)) {       // OpenCV's early-out refers to the grid
-      if (ymax > G - 1) ymax = G - 1;
-      struct { int idx, di; long long x, dx; long long ye; } e[2];
-      e[0].idx = e[1].idx = imin; e[0].ye = e[1].ye = ymin; e[0].di = 1; e[1].di = 3;
-      e[0].x = e[1].x = -XYONE; e[0].dx = e[1].dx = 0;
-      int edges = 4;
-      long long y = ymin;
-      while (y <= ymax) {
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          if (y >= e[i].ye) {
-            int idx0 = e[i].idx, di = e[i].di, idx = (idx0 + di) & 3;
-            for (; edges-- > 0;) {
-              const long long ty = (pick4(vy, idx) + delta) >> XYS;
-              if (ty > y) {
-                const long long xs = pick4(vx, idx0), xe = pick4(vx, idx);
-                e[i].ye = ty; e[i].dx = ((xe - xs) * 2 + (ty - y)) / (2 * (ty - y)); e[i].x = xs; e[i].idx = idx;
-                break;
-              }
-              idx0 = idx; idx = (idx + di) & 3;
-            }
-          }
-        }
-        if (edges < 0) break;
-        // rows y .. yn-1 use the current pair of edges (the serial loop re-examines an edge only when y reaches its ye)
-        long long yn = e[0].ye < e[1].ye ? e[0].ye : e[1].ye;
-        if (yn > ymax + 1) yn = ymax + 1;
-        if (yn <= y) yn = y + 1;
-        for (long long yy = y + lane; yy < yn; yy += 32) {
-          const long long ex0 = e[0].x + (yy - y) * e[0].dx, ex1 = e[1].x + (yy - y) * e[1].dx;
-          const bool sw = ex0 > ex1;
-          long long xx1 = ((sw ? ex1 : ex0) + delta) >> XYS, xx2 = ((sw ? ex0 : ex1) + delta) >> XYS;
-          const long long wy = yy - oy;
-          if (yy >= 0 && wy >= 0 && wy < H) {
-            xx1 -= ox; xx2 -= ox;
-            for (long long x = xx1 < 0 ? 0 : xx1; x <= xx2 && x < W; ++x) cut[wy * W + x] = 1;
-          }
-        }
-        e[0].x += (yn - y) * e[0].dx; e[1].x += (yn - y) * e[1].dx;
-        y = yn;
-      }
-    }
-  }
-  // Circle(center, 1, filled) at both (clipped) ends
-  if (lane < 2) {
-    const long long cx = lane ? px1 : px0, cy = lane ? py1 : py0;
-    put_px(cw, cx, cy); put_px(cw, cx - 1, cy); put_px(cw, cx + 1, cy);
-    put_px(cw, cx, cy - 1); put_px(cw, cx, cy + 1);
-  }
+  cvr::line(CutWin{cut, W, H, ox, oy}, G, r.x + ox, r.y + oy, r.z + ox, r.w + oy, 2, lane);
 }
 
 __global__ void thick_rays_kernel(const ExEnv* __restrict__ envs) {

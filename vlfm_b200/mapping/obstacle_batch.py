@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from .. import _lib
+from . import render as _render
 from . import sframe as _sf
 
 MAX_FRONTIERS = 4096
@@ -81,6 +82,7 @@ class ObstacleMapBatch:
         self._rec_pin = torch.zeros(rec * batch, dtype=torch.uint8).pin_memory()      # explore records read by the captured upload node
         self._rec_ev = torch.cuda.Event()
         self._rec_used = False
+        self._draw: Optional[_render.DrawLists] = None
 
     # ---------------------------------------------------------------- helpers ----
     def _pinned(self) -> torch.Tensor:
@@ -260,6 +262,27 @@ class ObstacleMapBatch:
             return [np.array([]) for _ in range(n)]
         fr = self.frontiers[:n, :m].cpu().numpy()
         return [fr[i, : cnt[i]].copy() if cnt[i] else np.array([]) for i in range(n)]
+
+    def render(self, slots: Optional[torch.Tensor] = None, padding_color: Sequence[int] = (100, 100, 100),
+               draw_lists: Optional[Sequence[Sequence[Sequence[int]]]] = None) -> torch.Tensor:
+        """ObstacleMap.visualize frames of n environments: [n, G, G, 3] uint8 BGR on the device.  ``slots`` (int32 [n],
+        default 0..batch-1) picks the grids and frontier lists (read on the device, no host round trip);
+        ``padding_color`` is the reference's ``radius_padding_color``; ``draw_lists[i]`` holds the draw records
+        (mapping/render.py) painted onto frame i after the flip."""
+        n = self.batch if slots is None else int(slots.shape[0])
+        g = self.size
+        pad = [int(c) for c in padding_color]
+        out = torch.empty((n, g, g, 3), dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            rc = self.lib.vlfm_render_obstacle(g, n, _lib.ptr(slots), _lib.ptr(self.obst), _lib.ptr(self.nav), _lib.ptr(self.explored),
+                                               _lib.ptr(self.frontiers), _lib.ptr(self.count), MAX_FRONTIERS, pad[0], pad[1], pad[2],
+                                               _lib.ptr(out), _lib.stream_ptr())
+        _lib.check(rc, "vlfm_render_obstacle")
+        if draw_lists is not None:
+            if self._draw is None:
+                self._draw = _render.DrawLists(self.device)
+            self._draw.draw(out, draw_lists)
+        return out
 
     def px_to_xy(self, px: np.ndarray) -> np.ndarray:                              # base_map.py:48-60
         q = px.copy()

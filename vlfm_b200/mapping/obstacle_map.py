@@ -13,6 +13,7 @@ import numpy as np
 import torch
 
 from .. import _lib
+from . import render as _render
 from .base_map import BaseMap
 from .obstacle_batch import ObstacleMapBatch
 
@@ -134,14 +135,14 @@ class ObstacleMap(BaseMap):
                     if self._eng.index_error(0):
                         raise IndexError("obstacle cell index out of bounds for the map")
 
-    def visualize(self) -> np.ndarray:
-        """obstacle_map.py:171-193 (trajectory overlay omitted)."""
-        import cv2
+    def visualize_device(self) -> torch.Tensor:
+        """obstacle_map.py:171-193 on the device: [G, G, 3] uint8 BGR tensor with the frontier circles and the trajectory."""
+        recs = _render.trajectory_records(self._camera_positions, self._last_camera_yaw, self.pixels_per_meter, self._episode_pixel_origin)
+        return self._eng.render(padding_color=self.radius_padding_color, draw_lists=[recs])[0]
 
-        vis = np.ones((self.size, self.size, 3), dtype=np.uint8) * 255
-        vis[self.explored_area == 1] = (200, 255, 200)
-        vis[self._navigable_map == 0] = self.radius_padding_color
-        vis[self._map == 1] = (0, 0, 0)
-        for f in self._frontiers_px:
-            cv2.circle(vis, tuple([int(i) for i in f]), 5, (200, 0, 0), 2)
-        return cv2.flip(vis, 0)
+    def visualize(self) -> np.ndarray:
+        """obstacle_map.py:171-193 as a host [G, G, 3] uint8 array."""
+        self._eng.check_fill(0)
+        if int(self._eng.ex_status[0].item()) != 0:
+            raise _lib.VlfmError("explore: a device scratch buffer overflowed (too many contours / points)")
+        return self.visualize_device().cpu().numpy()

@@ -4,7 +4,8 @@ Reference: vlfm/mapping/value_map.py (class :33, update_map :100, sort_waypoints
 reset :96).  State lives in HBM (``conf [B,G,G] f32``, ``value [B,G,G,C] f32``); the
 per-step work is two CUDA launches through the C-ABI (csrc/value_map.cu).  Host-side
 work is argument marshalling only; numpy views of the grids are produced lazily
-(``_map`` / ``_value_map`` properties synchronise and copy device -> host).
+(``_map`` / ``_value_map`` properties synchronise and copy device -> host).  ``visualize`` renders on the device
+(csrc/render.cu, mapping/render.py).
 """
 from __future__ import annotations
 
@@ -16,6 +17,7 @@ import numpy as np
 import torch
 
 from .. import _lib
+from . import render as _render
 from .base_map import BaseMap
 
 MIN_CONFIDENCE = 0.25  # value_map.py:40
@@ -67,6 +69,11 @@ def _disc(radius: int, device: torch.device) -> torch.Tensor:
     return _DISCS[key]
 
 
+def max_channels(i: np.ndarray) -> np.ndarray:
+    """ValueMap.visualize's default reduce_fn (value_map.py:192); passing this function keeps the reduction on the device."""
+    return np.max(i, axis=-1)
+
+
 def fusion_code(use_max_confidence: bool, fusion_type: str) -> int:
     if fusion_type == "replace":
         return _lib.FUSE_REPLACE
@@ -96,6 +103,12 @@ class ValueMapBatch:
         self._ws: Optional[torch.Tensor] = None
         self._ws_key: Optional[Tuple[int, int, int]] = None
         self.rows_per_tile = 0
+        # The reference's value grid becomes float64 in the first fuse of a weighted map (value_map.py:423) and stays so
+        # through reset(); before that fuse it is all zero, which renders white in either dtype.  Frames of such maps are
+        # therefore normalised in float64 (an exact upcast of the float32 grid), all others in float32.
+        self.ref_float64 = self.fusion in (_lib.FUSE_WEIGHTED, _lib.FUSE_WEIGHTED | _lib.FUSE_EQUAL)
+        self._render_ws = _render._Workspace()
+        self._draw: Optional[_render.DrawLists] = None
 
     def _params(self, h: int, w: int, min_depth: float, max_depth: float) -> "_lib.ValueParams":
         side = 2 * int(max_depth * self.ppm) + 1
@@ -163,6 +176,25 @@ class ValueMapBatch:
                                                        _lib.ptr(_disc(radius, self.device)), _lib.ptr(out), _lib.stream_ptr())
         _lib.check(rc, "vlfm_value_disc_median_batch")
         return out.cpu().numpy()
+
+    def render(self, slots: Optional[torch.Tensor] = None, reduced: Optional[torch.Tensor] = None, explored: Optional[torch.Tensor] = None,
+               draw_lists: Optional[Sequence[Sequence[Sequence[int]]]] = None) -> torch.Tensor:
+        """ValueMap.visualize frames of n environments: [n, G, G, 3] uint8 BGR on the device.  ``slots`` (int32 [n], default
+        0..batch-1) picks the grids; ``reduced`` [n, G, G] float32 / float64 replaces the default reduction value.amax(-1);
+        ``explored`` [nslots, G, G] uint8 (read at the same slots) zeroes unexplored cells; ``draw_lists[i]`` holds the draw
+        records (mapping/render.py) painted onto frame i in order."""
+        if reduced is None:
+            v = self.value if slots is None else self.value[slots.long()]
+            reduced = v.amax(-1)
+            if self.ref_float64:
+                reduced = reduced.double()
+        reduced = reduced.contiguous()
+        frames = _render.value_frames(reduced, explored, slots, self._render_ws)
+        if draw_lists is not None:
+            if self._draw is None:
+                self._draw = _render.DrawLists(self.device)
+            self._draw.draw(frames, draw_lists)
+        return frames
 
     def reset(self, slot: Optional[int] = None) -> None:
         if slot is None:
@@ -300,19 +332,29 @@ class ValueMap(BaseMap):
         order = np.argsort([-v for v in values])
         return np.array([waypoints[i] for i in order]), [values[i] for i in order]
 
-    def visualize(self, markers=None, reduce_fn: Callable = lambda i: np.max(i, axis=-1), obstacle_map=None) -> np.ndarray:
-        """value_map.py:189-219 (inferno rendering of the reduced map; trajectory overlay omitted)."""
-        import cv2
+    def visualize_device(self, markers: Optional[List[Tuple[np.ndarray, Dict[str, Any]]]] = None,
+                         reduce_fn: Callable = max_channels, obstacle_map: Optional[Any] = None) -> torch.Tensor:
+        """value_map.py:189-219 on the device: [G, G, 3] uint8 BGR tensor (csrc/render.cu).  The default reduce_fn reduces
+        on the device; any other callable runs on the host, as in the reference, on the value grid in the dtype the
+        reference's grid has (``ValueMapBatch.ref_float64``), and its result is uploaded."""
+        reduced = None
+        if reduce_fn is not max_channels:
+            grid = self._value_map
+            if self._eng.ref_float64:
+                grid = grid.astype(np.float64)
+            red = np.asarray(reduce_fn(grid))
+            if red.dtype not in (np.float32, np.float64):
+                red = red.astype(np.float64)
+            reduced = torch.from_numpy(np.ascontiguousarray(red)).to(self.device)[None]
+        recs: List[List[int]] = []
+        if len(self._camera_positions) > 0:           # no trajectory: neither the agent nor the markers (:208-217)
+            recs = _render.trajectory_records(self._camera_positions, self._last_camera_yaw, self.pixels_per_meter,
+                                              self._episode_pixel_origin)
+            recs += _render.marker_records(markers, self.pixels_per_meter, self._episode_pixel_origin)
+        explored = obstacle_map.explored_device() if obstacle_map is not None else None
+        return self._eng.render(reduced=reduced, explored=explored, draw_lists=[recs])[0]
 
-        reduced = reduce_fn(self._value_map).copy()
-        if obstacle_map is not None:
-            reduced[obstacle_map.explored_area == 0] = 0
-        img = np.flipud(reduced)
-        zero = img == 0
-        img = img.copy()
-        img[zero] = np.max(img)
-        lo, hi = float(img.min()), float(img.max())
-        norm = ((img - lo) / (hi - lo) * 255).astype(np.uint8) if hi > lo else np.zeros_like(img, np.uint8)
-        rgb = cv2.applyColorMap(norm, cv2.COLORMAP_INFERNO)
-        rgb[zero] = (255, 255, 255)
-        return rgb
+    def visualize(self, markers: Optional[List[Tuple[np.ndarray, Dict[str, Any]]]] = None, reduce_fn: Callable = max_channels,
+                  obstacle_map: Optional[Any] = None) -> np.ndarray:
+        """value_map.py:189-219: the inferno frame with the trajectory and the markers, as a host [G, G, 3] uint8 array."""
+        return self.visualize_device(markers, reduce_fn, obstacle_map).cpu().numpy()
