@@ -398,6 +398,57 @@ int vlfm_render_obstacle(int G, int batch, const int32_t* d_slots, const uint8_t
 int vlfm_render_draw(int G, int batch, uint8_t* d_frames, const int32_t* h_lists, size_t list_ints, int32_t* d_lists,
                      size_t d_list_ints, void* stream);
 
+/* ------------------------------------------------------------------ MobileSAM ---- */
+/* Replaces MobileSAM.segment_bbox (vlfm/vlm/sam.py:40-57: SamPredictor.set_image + predict(box, multimask_output=False)) with the
+ * TinyViT-5M encoder and the box-prompted mask decoder (engine: vlfm_b200/vlm/sam_engine.py).  GEMMs, LayerNorms and the 7-key
+ * attentions run on vlfm_gemm_f16 / vlfm_gemm_f16_resid_ln / vlfm_layernorm / vlfm_attention_f16; these are the rest.
+ *
+ * vlfm_sam_preprocess: ResizeLongestSide(S): Pillow-exact bilinear resize [B,H,W,3] uint8 -> (OH, OW) (tables as for
+ *   vlfm_preprocess_im2col, built by vlm/preprocess.py::bilinear_tables; d_mid [B,H,OW,3] uint8 scratch), then
+ *   (x - mean) / std in fp32 (h_mean3 / h_std3: HOST float[3] on the 0..255 scale) and a zero pad to S x S -> d_out [B,S,S,3] fp16.
+ * vlfm_sam_im2col3x3: fp16 NHWC [B,H,W,C] -> fp16 [B*Ho*Wo, ldk] rows of a 3x3 conv (pad 1, stride 1 or 2), column (ky*3+kx)*C + c,
+ *   columns >= 9*C zero.  ldk % 8 == 0.
+ * vlfm_sam_dwconv3x3: depthwise 3x3 conv (pad 1, stride 1 or 2), NHWC, weights d_w [9, C] (tap-major, BatchNorm folded) + d_b [C],
+ *   then GELU when gelu != 0.  Input and output are fp32 (flag 1) or fp16 (0).
+ * vlfm_sam_add_act: out = act(a + b) over n elements (b may be NULL; act = GELU when gelu != 0) -> d_out32 and / or d_out16.
+ * vlfm_sam_window_attention: TinyViT window attention, head dim 32 (C = heads * 32), window ws in {7, 14}.  d_qkv [B*H*W, 3C] fp16
+ *   with columns [q | k | v], head h at h*32 inside each; d_pad_qkv [3C] fp16: the q/k/v row of a padding token (the map is
+ *   zero-padded to a window multiple before the attention's LayerNorm, so padded tokens are unmasked keys with this value);
+ *   d_bias [heads, ws*ws] fp32 indexed by |dy|*ws + |dx|.  d_out [B*H*W, C] fp16.
+ * vlfm_sam_box_tokens: decoder input tokens [M*7, D] fp32: rows 0..4 = d_fixed rows 0..4 (iou token, mask tokens), rows 5, 6 = the
+ *   random-Fourier encoding of the box corners (d_boxes [M,4] float64 x1,y1,x2,y2 in frame pixels, scaled to (newh, neww) in
+ *   float64, cast to float32, +0.5, / S; d_gauss [2, D/2]) plus d_fixed rows 5, 6 (corner embeddings).
+ * vlfm_sam_add_pe_f16: out16 = fp16(x), outp16 = fp16(x + pe[row % pe_rows]) over [rows, D]; either output may be NULL.
+ * vlfm_sam_decoder_init: d_keys [M, HW, D] = d_emb[d_frame[m]] + d_nomask (NaN rows for a frame index outside [0, F)).
+ * vlfm_sam_t2i_attention: softmax(scale q k^T) v per (box, head), head dim 16, Nq <= 8 queries per box, Nk keys per box; keys are
+ *   split over CTAs in 256-key chunks whose (max, sum, acc) go to d_part (M*heads*ceil(Nk/256)*Nq*18 floats) and are merged in
+ *   chunk order by a second launch: bitwise reproducible, no atomics.
+ * vlfm_sam_pixel_shuffle2: d_in [B*h*w, 4*C] fp32 (column (dy*2+dx)*C + c: the GEMM of a 2x2 stride-2 transposed conv)
+ *   -> d_out [B, 2h, 2w, C].
+ * vlfm_sam_mask_logits: d_logits [M, 2h, 2w] = sum_c d_hyper[m,c] * GELU(second transposed conv, d_up laid out as above).
+ * vlfm_sam_mask_finish: low-res logits [M, L, L] -> bilinear (align_corners=False) to S x S -> crop [:newh, :neww] -> bilinear
+ *   to (H, W) -> > 0 -> d_out [M, H, W] uint8. */
+int vlfm_sam_preprocess(const uint8_t* d_img, uint8_t* d_mid, void* d_out, int B, int H, int W, int OH, int OW, int S,
+                        const int32_t* d_hbounds, const int32_t* d_hkk, int hksize, const int32_t* d_vbounds, const int32_t* d_vkk,
+                        int vksize, const float* h_mean3, const float* h_std3, void* stream);
+int vlfm_sam_im2col3x3(const void* d_x16, void* d_col16, int B, int H, int W, int C, int stride, int ldk, void* stream);
+int vlfm_sam_dwconv3x3(const void* d_in, int in_f32, const float* d_w, const float* d_b, void* d_out, int out_f32, int B, int H, int W,
+                       int C, int stride, int gelu, void* stream);
+int vlfm_sam_add_act(const float* d_a, const float* d_b, float* d_out32, void* d_out16, long long n, int gelu, void* stream);
+int vlfm_sam_window_attention(const void* d_qkv, const void* d_pad_qkv, const float* d_bias, void* d_out, int B, int H, int W, int C,
+                              int heads, int ws, float scale, void* stream);
+int vlfm_sam_box_tokens(const double* d_boxes, int M, int H, int W, int newh, int neww, int S, const float* d_gauss, const float* d_fixed,
+                        float* d_tokens, int D, void* stream);
+int vlfm_sam_add_pe_f16(const float* d_x, const float* d_pe, void* d_out16, void* d_outp16, long long rows, long long pe_rows, int D,
+                        void* stream);
+int vlfm_sam_decoder_init(const float* d_emb, const int32_t* d_frame, const float* d_nomask, float* d_keys, int M, int F, int HW, int D,
+                          void* stream);
+int vlfm_sam_t2i_attention(const void* d_q, const void* d_k, const void* d_v, void* d_o, int M, int heads, int Nq, int Nk, int ldq,
+                           int ldk, int ldv, int ldo, float scale, float* d_part, size_t part_floats, void* stream);
+int vlfm_sam_pixel_shuffle2(const float* d_in, float* d_out, int B, int h, int w, int C, void* stream);
+int vlfm_sam_mask_logits(const float* d_up, const float* d_hyper, float* d_logits, int M, int h, int w, int C, void* stream);
+int vlfm_sam_mask_finish(const float* d_low, uint8_t* d_out, int M, int L, int S, int newh, int neww, int H, int W, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

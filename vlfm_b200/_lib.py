@@ -109,6 +109,19 @@ _SIGNATURES = {
     "vlfm_render_value": (C.c_int, [C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P, C.c_size_t, _P]),
     "vlfm_render_obstacle": (C.c_int, [C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "vlfm_render_draw": (C.c_int, [C.c_int, C.c_int, _P, _P, C.c_size_t, _P, C.c_size_t, _P]),
+    "vlfm_sam_preprocess": (C.c_int, [_P, _P, _P] + [C.c_int] * 6 + [_P, _P, C.c_int, _P, _P, C.c_int,
+                                      C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
+    "vlfm_sam_im2col3x3": (C.c_int, [_P, _P] + [C.c_int] * 6 + [_P]),
+    "vlfm_sam_dwconv3x3": (C.c_int, [_P, C.c_int, _P, _P, _P] + [C.c_int] * 7 + [_P]),
+    "vlfm_sam_add_act": (C.c_int, [_P, _P, _P, _P, C.c_longlong, C.c_int, _P]),
+    "vlfm_sam_window_attention": (C.c_int, [_P, _P, _P, _P] + [C.c_int] * 6 + [C.c_float, _P]),
+    "vlfm_sam_box_tokens": (C.c_int, [_P] + [C.c_int] * 6 + [_P, _P, _P, C.c_int, _P]),
+    "vlfm_sam_add_pe_f16": (C.c_int, [_P, _P, _P, _P, C.c_longlong, C.c_longlong, C.c_int, _P]),
+    "vlfm_sam_decoder_init": (C.c_int, [_P, _P, _P, _P] + [C.c_int] * 4 + [_P]),
+    "vlfm_sam_t2i_attention": (C.c_int, [_P, _P, _P, _P] + [C.c_int] * 8 + [C.c_float, _P, C.c_size_t, _P]),
+    "vlfm_sam_pixel_shuffle2": (C.c_int, [_P, _P] + [C.c_int] * 4 + [_P]),
+    "vlfm_sam_mask_logits": (C.c_int, [_P, _P, _P] + [C.c_int] * 4 + [_P]),
+    "vlfm_sam_mask_finish": (C.c_int, [_P, _P] + [C.c_int] * 7 + [_P]),
 }
 
 _lib = None

@@ -56,11 +56,39 @@ def bicubic_tables(in_size: int, out_size: int) -> Tuple[np.ndarray, np.ndarray,
     return bounds, kk, ksize
 
 
-def resize_numpy(img: np.ndarray, out_h: int, out_w: int) -> np.ndarray:
+def _bilinear(x: float) -> float:
+    x = abs(x)
+    return 1.0 - x if x < 1.0 else 0.0
+
+
+@lru_cache(maxsize=None)
+def bilinear_tables(in_size: int, out_size: int) -> Tuple[np.ndarray, np.ndarray, int]:
+    """Pillow's BILINEAR (support 1) tables in the layout of ``bicubic_tables`` (MobileSAM's ResizeLongestSide)."""
+    scale = in_size / out_size
+    filterscale = max(scale, 1.0)
+    support = 1.0 * filterscale
+    ksize = int(math.ceil(support)) * 2 + 1
+    bounds = np.zeros((out_size, 2), np.int32)
+    kk = np.zeros((out_size, ksize), np.int32)
+    ss = 1.0 / filterscale
+    for xx in range(out_size):
+        center = (xx + 0.5) * scale
+        xmin = max(int(center - support + 0.5), 0)
+        xmax = min(int(center + support + 0.5), in_size) - xmin
+        w = [_bilinear((x + xmin - center + 0.5) * ss) for x in range(xmax)]
+        ww = sum(w)
+        for x in range(xmax):
+            k = w[x] / ww if ww != 0.0 else w[x]
+            kk[xx, x] = int(-0.5 + k * (1 << PRECISION_BITS)) if k < 0 else int(0.5 + k * (1 << PRECISION_BITS))
+        bounds[xx] = (xmin, xmax)
+    return bounds, kk, ksize
+
+
+def resize_numpy(img: np.ndarray, out_h: int, out_w: int, tables=bicubic_tables) -> np.ndarray:
     """Reference emulation of the two GPU passes (used by CPU tests to pin the tables to PIL)."""
     h, w, _ = img.shape
-    hb, hk, _ = bicubic_tables(w, out_w)
-    vb, vk, _ = bicubic_tables(h, out_h)
+    hb, hk, _ = tables(w, out_w)
+    vb, vk, _ = tables(h, out_h)
     src = img.astype(np.int64)
     mid = np.zeros((h, out_w, 3), np.int64)
     for xo in range(out_w):
