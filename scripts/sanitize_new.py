@@ -5,7 +5,8 @@ import numpy as np, torch
 from vlfm_b200.mapping.obstacle_map import ObstacleMap
 from vlfm_b200.mapping.value_map import build_cone_template
 from vlfm_b200.utils.synthetic import focal_from_hfov, trajectory
-from vlfm_b200.vlm.gdino_accel import TcMSDA, cast_f16
+from vlfm_b200.vlm.dense import cast_f16
+from vlfm_b200.vlm.gdino_accel import TcMSDA
 from vlfm_b200 import _lib
 import ctypes
 

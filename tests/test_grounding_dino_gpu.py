@@ -87,7 +87,8 @@ def test_msda_kernel_vs_torch_grid_sample(f16):
 
 
 def test_tc_linear_and_cast_vs_torch():
-    from vlfm_b200.vlm.gdino_accel import TcLinear, cast_f16
+    from vlfm_b200.vlm.dense import cast_f16
+    from vlfm_b200.vlm.gdino_accel import TcLinear
 
     torch.manual_seed(1)
     x = torch.randn(3, 1001, 256, device="cuda")

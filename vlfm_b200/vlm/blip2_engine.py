@@ -13,12 +13,13 @@ from __future__ import annotations
 import ctypes
 import math
 import os
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from .. import _lib
+from . import dense
 from .blip2_config import Blip2Dims
 from .preprocess import CLIP_MEAN, CLIP_STD, bicubic_tables
 
@@ -49,16 +50,15 @@ class Blip2ITCEngine:
         self._tables: Dict[Tuple[int, int], Tuple[torch.Tensor, ...]] = {}
         self._mean = (ctypes.c_float * 3)(*CLIP_MEAN)
         self._std = (ctypes.c_float * 3)(*CLIP_STD)
-        # Q-Former in float32-grade arithmetic (x2 operands on the fp16 tensor path, fp32 attention): the reference runs it in fp32
-        # (only the ViT is half precision in lavis) and fp16 operands there alone cost ~3e-5 on the cosine.  VLFM_QFORMER_X2=0: fp16.
-        self.x2 = os.environ.get("VLFM_QFORMER_X2", "1") != "0"
+        # the Q-Former runs in float32-grade arithmetic (x2 operands on the fp16 tensor path, fp32 attention): the reference runs it
+        # in fp32 (only the ViT is half precision in lavis) and fp16 operands there alone cost ~3e-5 on the cosine
         self._load(state_dict)
         self._alloc(max_batch)
         self.text_feat = torch.zeros(dims.proj, dtype=F32, device=self.dev)
         # residual GEMM + LayerNorm as one C-ABI call with a deterministic split-K reduction (partial sums stored side by side, added
-        # to the residual stream in split order by the LayerNorm launch): the cosine is bitwise reproducible run to run.
-        # VLFM_DET_SPLITK=0 restores round 1's red.global.add reduction (order of arrival, ~6e-5 spread on the cosine).
-        self.fuse_ln = os.environ.get("VLFM_DET_SPLITK", "1") != "0"
+        # to the residual stream in split order by the LayerNorm launch): the cosine is bitwise reproducible run to run.  False runs
+        # them as a plain residual GEMM (self._gemm / self._gemm_x2) and a LayerNorm launch: bench.py's GEMM replay records them so.
+        self.fuse_ln = True
         self._partials = torch.empty(partials_floats(dims, max_batch), dtype=F32, device=self.dev)
         self._fold_layer0()
         self._many_out: Dict[int, torch.Tensor] = {}   # forward_many / head outputs [max_batch, P], one per P
@@ -128,34 +128,20 @@ class Blip2ITCEngine:
                 L["cln_w"], L["cln_b"] = f(sd[c + "output.LayerNorm.weight"]), f(sd[c + "output.LayerNorm.bias"])
                 kv_w.append(torch.cat([sd[c + "attention.key.weight"], sd[c + "attention.value.weight"]], 0))
                 kv_b.append(torch.cat([sd[c + "attention.key.bias"], sd[c + "attention.value.bias"]], 0))
-            if self.x2:
-                srcs = {"qkv_w": torch.cat([sd[a + "attention.query.weight"], sd[a + "attention.key.weight"], sd[a + "attention.value.weight"]], 0),
-                        "so_w": sd[a + "output.dense.weight"], "iq_w": sd[p + "intermediate_query.dense.weight"],
-                        "oq_w": sd[p + "output_query.dense.weight"], "it_w": sd[p + "intermediate.dense.weight"], "ot_w": sd[p + "output.dense.weight"]}
-                if L["cross"] >= 0:
-                    srcs["cq_w"], srcs["co_w"] = sd[c + "attention.query.weight"], sd[c + "output.dense.weight"]
-                for k_, w_ in srcs.items():
-                    L[k_ + "l"] = lo(w_)
+            srcs = {"qkv_w": torch.cat([sd[a + "attention.query.weight"], sd[a + "attention.key.weight"], sd[a + "attention.value.weight"]], 0),
+                    "so_w": sd[a + "output.dense.weight"], "iq_w": sd[p + "intermediate_query.dense.weight"],
+                    "oq_w": sd[p + "output_query.dense.weight"], "it_w": sd[p + "intermediate.dense.weight"], "ot_w": sd[p + "output.dense.weight"]}
+            if L["cross"] >= 0:
+                srcs["cq_w"], srcs["co_w"] = sd[c + "attention.query.weight"], sd[c + "output.dense.weight"]
+            for k_, w_ in srcs.items():
+                L[k_ + "l"] = lo(w_)
             self.qf.append(L)
         self.ncross = len(kv_w)
         self.kv_w, self.kv_b = h(torch.cat(kv_w, 0)), f(torch.cat(kv_b, 0))  # one GEMM feeds every cross layer
         self.vp_w, self.vp_b = h(sd["vision_projection.weight"]), f(sd["vision_projection.bias"])
         self.tp_w, self.tp_b = h(sd["text_projection.weight"]), f(sd["text_projection.bias"])
-        if self.x2:
-            self.kv_wl, self.vp_wl, self.tp_wl = lo(torch.cat(kv_w, 0)), lo(sd["vision_projection.weight"]), lo(sd["text_projection.weight"])
-        # layernorm(query_tokens) is input independent (modeling: qformer.layernorm on query_embeds)
-        q0 = f(sd["query_tokens"].reshape(d.queries, H))
-        self.q0_32 = torch.empty_like(q0)
-        self.q0_16 = torch.empty(d.queries, H, dtype=F16, device=dev)
-        self.q0_lo = torch.empty(d.queries, H, dtype=F16, device=dev)
-        self._ln_x2(q0, self.q_ln_w, self.q_ln_b, self.q0_16, self.q0_lo, self.q0_32, d.q_eps)
-
-    def weight_bytes(self) -> int:
-        n = 0
-        for t in [self.patch_w, self.kv_w, self.vp_w] + ([self.kv_wl, self.vp_wl] if self.x2 else []) + [v for L in self.vit for k, v in L.items() if k.endswith("_w") and v.dtype == F16] \
-                + [v for L in self.qf for k, v in L.items() if isinstance(v, torch.Tensor) and v.dtype == F16 and k[:2] not in ("it", "ot")]:   # text-branch FFN weights are not on the per-image path
-            n += t.numel() * 2
-        return n
+        self.kv_wl, self.vp_wl, self.tp_wl = lo(torch.cat(kv_w, 0)), lo(sd["vision_projection.weight"]), lo(sd["text_projection.weight"])
+        self.query_tokens = f(sd["query_tokens"].reshape(d.queries, H))
 
     # ------------------------------------------------------------------ buffers ----
     def _alloc(self, B: int) -> None:
@@ -170,87 +156,45 @@ class Blip2ITCEngine:
         self.b_ao = e(B * T, D)
         self.b_h = e(B * T, Fv)
         self.b_img = e(B * T, D)
-        self.b_kv = e(B * T, self.ncross * 2 * H)
+        self.b_img32 = e(B * T, D, dt=F32)
+        self.b_img_lo = e(B * T, D)
+        self.b_kv32 = e(B * T, self.ncross * 2 * H, dt=F32)
+        # the Q-Former's activations: x2 operand pairs (hi, lo) and fp32 q / k / v
         self.q_h32 = e(B * Q, H, dt=F32)
         self.q_h16 = e(B * Q, H)
-        self.q_qkv = e(B * Q, 3 * H)
-        self.q_q = e(B * Q, H)
+        self.q_h_lo = e(B * Q, H)
+        self.q_qkv32 = e(B * Q, 3 * H, dt=F32)
+        self.q_q32 = e(B * Q, H, dt=F32)
         self.q_ao = e(B * Q, H)
+        self.q_ao_lo = e(B * Q, H)
         self.q_f = e(B * Q, I)
+        self.q_f_lo = e(B * Q, I)
         self.q_proj = e(B * Q, d.proj, dt=F32)
-        if self.x2:
-            self.b_img32 = e(B * T, D, dt=F32)
-            self.b_img_lo = e(B * T, D)
-            self.b_kv32 = e(B * T, self.ncross * 2 * H, dt=F32)
-            self.q_h_lo = e(B * Q, H)
-            self.q_qkv32 = e(B * Q, 3 * H, dt=F32)
-            self.q_q32 = e(B * Q, H, dt=F32)
-            self.q_ao_lo = e(B * Q, H)
-            self.q_f_lo = e(B * Q, I)
         self.out = torch.zeros(B, dtype=F32, device=dev)
 
     # ---------------------------------------------------------------- primitives ----
+    # _gemm / _gemm_x2 stay methods: bench.py's GEMM replay swaps them for recording wrappers (with fuse_ln off, every GEMM of the
+    # forward goes through them)
     def _gemm(self, a, w, bias, epi, out):
-        M, K = a.shape
-        rc = self.lib.vlfm_gemm_f16(a.data_ptr(), w.data_ptr(), _lib.ptr(bias), out.data_ptr(), M, w.shape[0], K,
-                                    a.stride(0), w.stride(0), out.stride(0), epi, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_gemm_f16")
+        dense.gemm_f16(a, w, bias, epi, out)
+
+    def _gemm_x2(self, a, al, w, wl, bias, epi, out, out_lo=None):
+        dense.gemm_f16x2(a, al, w, wl, bias, epi, out, out_lo)
 
     def _gemm_resid_ln(self, a, w, bias, x, g, b, out16, out32, eps):
         """x += a @ w^T + bias ; LayerNorm(x) -> out16 / out32 (GEMM launch + reduce/LayerNorm launch, bitwise reproducible)."""
         if not self.fuse_ln:
             self._gemm(a, w, bias, _lib.EPI_BIAS_RESID_F32, x)
-            self._ln(x, g, b, out16, out32, eps)
+            dense.layernorm(x, g, b, eps, out16, out32)
             return
-        M, K = a.shape
-        rc = self.lib.vlfm_gemm_f16_resid_ln(a.data_ptr(), w.data_ptr(), _lib.ptr(bias), x.data_ptr(), M, w.shape[0], K, a.stride(0),
-                                             w.stride(0), x.stride(0), g.data_ptr(), b.data_ptr(), _lib.ptr(out16),
-                                             out16.stride(0) if out16 is not None else 0, _lib.ptr(out32),
-                                             out32.stride(0) if out32 is not None else 0, eps, self._partials.data_ptr(),
-                                             self._partials.numel() * 4, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_gemm_f16_resid_ln")
-
-    def _gemm_x2(self, a, al, w, wl, bias, epi, out, out_lo=None):
-        """x2 operands (hi, lo) on both sides -> fp32 (EPI_BIAS_F32 / EPI_BIAS_RESID_F32) or GELU + x2 operands (EPI_BIAS_GELU_F16X2)"""
-        M, K = a.shape
-        rc = self.lib.vlfm_gemm_f16x2(a.data_ptr(), al.data_ptr(), w.data_ptr(), wl.data_ptr(), _lib.ptr(bias), out.data_ptr(), _lib.ptr(out_lo),
-                                      M, w.shape[0], K, a.stride(0), w.stride(0), out.stride(0), epi, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_gemm_f16x2")
+        dense.gemm_f16_resid_ln(a, w, bias, x, g, b, eps, out16, out32, partials=self._partials)
 
     def _gemm_x2_resid_ln(self, a, al, w, wl, bias, x, g, b, out_hi, out_lo, out32, eps):
         if not self.fuse_ln:
             self._gemm_x2(a, al, w, wl, bias, _lib.EPI_BIAS_RESID_F32, x)
-            self._ln_x2(x, g, b, out_hi, out_lo, out32, eps)
+            dense.layernorm_x2(x, g, b, eps, out_hi, out_lo, out32)
             return
-        M, K = a.shape
-        rc = self.lib.vlfm_gemm_f16x2_resid_ln(a.data_ptr(), al.data_ptr(), w.data_ptr(), wl.data_ptr(), _lib.ptr(bias), x.data_ptr(), M, w.shape[0], K,
-                                               a.stride(0), w.stride(0), x.stride(0), g.data_ptr(), b.data_ptr(), out_hi.data_ptr(), out_lo.data_ptr(),
-                                               out_hi.stride(0), _lib.ptr(out32), out32.stride(0) if out32 is not None else 0, eps,
-                                               self._partials.data_ptr(), self._partials.numel() * 4, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_gemm_f16x2_resid_ln")
-
-    def _ln_x2(self, x, g, b, out_hi, out_lo, out32, eps):
-        rows, D = x.shape
-        rc = self.lib.vlfm_layernorm_x2(x.data_ptr(), g.data_ptr(), b.data_ptr(), out_hi.data_ptr(), out_lo.data_ptr(), _lib.ptr(out32), rows, D,
-                                        x.stride(0), out_hi.stride(0), out32.stride(0) if out32 is not None else 0, eps, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_layernorm_x2")
-
-    def _attn32(self, q, k, v, o_hi, o_lo, B, heads, Nq, Nk, hd, scale):
-        rc = self.lib.vlfm_attention_f32(q.data_ptr(), k.data_ptr(), v.data_ptr(), o_hi.data_ptr(), o_lo.data_ptr(), B, heads, Nq, Nk, hd,
-                                         q.stride(0), k.stride(0), v.stride(0), o_hi.stride(0), scale, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_attention_f32")
-
-    def _ln(self, x, g, b, out16, out32, eps):
-        rows, D = x.shape
-        rc = self.lib.vlfm_layernorm(x.data_ptr(), g.data_ptr(), b.data_ptr(), _lib.ptr(out16), _lib.ptr(out32), rows, D,
-                                     x.stride(0), out16.stride(0) if out16 is not None else 0,
-                                     out32.stride(0) if out32 is not None else 0, eps, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_layernorm")
-
-    def _attn(self, q, k, v, o, B, heads, Nq, Nk, hd, scale):
-        rc = self.lib.vlfm_attention_f16(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), B, heads, Nq, Nk, hd,
-                                         q.stride(0), k.stride(0), v.stride(0), o.stride(0), scale, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_attention_f16")
+        dense.gemm_f16x2_resid_ln(a, al, w, wl, bias, x, g, b, eps, out_hi, out_lo, out32, partials=self._partials)
 
     def _resize_tables(self, h: int, w: int):
         key = (h, w)
@@ -279,94 +223,59 @@ class Blip2ITCEngine:
         _lib.check(rc, "vlfm_assemble_tokens")
         x, xn, qkv, ao, hb_ = self.b_x[:n], self.b_xn[:n], self.b_qkv[:n], self.b_ao[:n], self.b_h[:n]
         hd = D // d.v_heads
-        img16 = self.b_img[:n]
-        self._ln(x, self.vit[0]["ln1_w"], self.vit[0]["ln1_b"], xn, None, d.v_eps)
+        img16, img32 = self.b_img[:n], self.b_img32[:n]
+        dense.layernorm(x, self.vit[0]["ln1_w"], self.vit[0]["ln1_b"], d.v_eps, xn)
         for i, L in enumerate(self.vit):
             self._gemm(xn, L["qkv_w"], L["qkv_b"], _lib.EPI_BIAS_F16, qkv)
-            self._attn(qkv[:, 0:D], qkv[:, D : 2 * D], qkv[:, 2 * D : 3 * D], ao, B, d.v_heads, T, T, hd, hd**-0.5)
+            dense.attention_f16(qkv[:, 0:D], qkv[:, D : 2 * D], qkv[:, 2 * D : 3 * D], B, d.v_heads, T, T, hd, hd**-0.5, ao)
             self._gemm_resid_ln(ao, L["proj_w"], L["proj_b"], x, L["ln2_w"], L["ln2_b"], xn, None, d.v_eps)
             self._gemm(xn, L["fc1_w"], L["fc1_b"], _lib.EPI_BIAS_GELU_F16, hb_)
             if i + 1 < len(self.vit):   # the next block's pre-norm rides on this block's residual GEMM
                 nx = self.vit[i + 1]
                 self._gemm_resid_ln(hb_, L["fc2_w"], L["fc2_b"], x, nx["ln1_w"], nx["ln1_b"], xn, None, d.v_eps)
             else:                       # ... and the post-LayerNorm on the last one
-                self._gemm_resid_ln(hb_, L["fc2_w"], L["fc2_b"], x, self.post_w, self.post_b, img16, self.b_img32[:n] if self.x2 else None, d.v_eps)
-        h32, h16 = self.q_h32[:nq], self.q_h16[:nq]
-        if not (self.x2 and self.fold0):
-            h32.view(B, Q, H).copy_(self.q0_32)
-            h16.view(B, Q, H).copy_(self.q0_16)
-        if self.x2:
-            # image embeds as x2 operands: hi is the fp16 LayerNorm output itself, lo its residual against the fp32 one
-            img_lo = self.b_img_lo[:n]
-            _lib.check(self.lib.vlfm_split_x2(self.b_img32.data_ptr(), 0, img_lo.data_ptr(), n * D, _lib.stream_ptr()), "vlfm_split_x2")
-            kv = self.b_kv32[:n]
-            self._gemm_x2(img16, img_lo, self.kv_w, self.kv_wl, self.kv_b, _lib.EPI_BIAS_F32, kv)
-            hlo = self.q_h_lo[:nq]
-            if self.fold0:      # only the residual stream needs its start value: hhi / hlo are rewritten by layer 0's cross block
-                h32.copy_(self.f0_32x[:nq])
-            else:
-                hlo.view(B, Q, H).copy_(self.q0_lo)
-            self._qformer_layers_x2(h32, h16, hlo, B, Q, kv, T, text=False, folded=self.fold0)
-            self._gemm_x2(h16, hlo, self.vp_w, self.vp_wl, self.vp_b, _lib.EPI_BIAS_F32, self.q_proj[:nq])
-        else:
-            kv = self.b_kv[:n]
-            self._gemm(img16, self.kv_w, self.kv_b, _lib.EPI_BIAS_F16, kv)
-            self._qformer_layers(h32, h16, B, Q, kv, T, text=False)
-            self._gemm(h16, self.vp_w, self.vp_b, _lib.EPI_BIAS_F32, self.q_proj[:nq])
+                self._gemm_resid_ln(hb_, L["fc2_w"], L["fc2_b"], x, self.post_w, self.post_b, img16, img32, d.v_eps)
+        # image embeds as x2 operands: hi is the fp16 LayerNorm output itself, lo its residual against the fp32 one
+        img_lo = self.b_img_lo[:n]
+        dense.split_x2(img32, img_lo)
+        kv = self.b_kv32[:n]
+        self._gemm_x2(img16, img_lo, self.kv_w, self.kv_wl, self.kv_b, _lib.EPI_BIAS_F32, kv)
+        # layer 0's self-attention block is folded (_fold_layer0): only the residual stream needs its start value, the x2 operands
+        # are rewritten by layer 0's cross block
+        h32, hhi, hlo = self.q_h32[:nq], self.q_h16[:nq], self.q_h_lo[:nq]
+        h32.copy_(self.f0_32x[:nq])
+        self._qformer_layers(h32, hhi, hlo, B, Q, kv, T, text=False)
+        self._gemm_x2(hhi, hlo, self.vp_w, self.vp_wl, self.vp_b, _lib.EPI_BIAS_F32, self.q_proj[:nq])
         rc = self.lib.vlfm_itc_head(self.q_proj.data_ptr(), self.text_feat.data_ptr(), self.out.data_ptr(), B, Q, d.proj,
                                     _lib.stream_ptr())
         _lib.check(rc, "vlfm_itc_head")
 
-    def _qformer_layers(self, h32, h16, B, S, kv, T, text: bool) -> None:
-        d = self.d
-        H = d.q_hidden
-        hd = H // d.q_heads
-        n = B * S
-        qkv, qq, ao, ff = self.q_qkv[:n], self.q_q[:n], self.q_ao[:n], self.q_f[:n]
-        sc = 1.0 / math.sqrt(hd)
-        for L in self.qf:
-            self._gemm(h16, L["qkv_w"], L["qkv_b"], _lib.EPI_BIAS_F16, qkv)
-            self._attn(qkv[:, 0:H], qkv[:, H : 2 * H], qkv[:, 2 * H : 3 * H], ao, B, d.q_heads, S, S, hd, sc)
-            self._gemm_resid_ln(ao, L["so_w"], L["so_b"], h32, L["sln_w"], L["sln_b"], h16, h32, d.q_eps)
-            if not text and L["cross"] >= 0:
-                j = L["cross"]
-                self._gemm(h16, L["cq_w"], L["cq_b"], _lib.EPI_BIAS_F16, qq)
-                self._attn(qq, kv[:, j * 2 * H : j * 2 * H + H], kv[:, j * 2 * H + H : (j + 1) * 2 * H], ao, B, d.q_heads, S, T, hd, sc)
-                self._gemm_resid_ln(ao, L["co_w"], L["co_b"], h32, L["cln_w"], L["cln_b"], h16, h32, d.q_eps)
-            iw, ib, ow, ob, lw, lb = ((L["it_w"], L["it_b"], L["ot_w"], L["ot_b"], L["otln_w"], L["otln_b"]) if text else
-                                      (L["iq_w"], L["iq_b"], L["oq_w"], L["oq_b"], L["oqln_w"], L["oqln_b"]))
-            self._gemm(h16, iw, ib, _lib.EPI_BIAS_GELU_F16, ff)
-            self._gemm_resid_ln(ff, ow, ob, h32, lw, lb, h16, h32, d.q_eps)
-
     def _fold_layer0(self) -> None:
-        """Layer 0's self-attention block sees only LayerNorm(query_tokens): it (and the query projection of layer 0's
-        cross-attention that follows it) is the same for every image -- computed once here with the step's own kernels."""
-        self.fold0 = False
-        if not self.x2:
-            return
+        """Layer 0's self-attention block sees only LayerNorm(query_tokens) (modeling: qformer.layernorm on query_embeds): it (and
+        the query projection of layer 0's cross-attention that follows it) is the same for every image -- computed once here with
+        the step's own kernels."""
         d = self.d
         Q, H = d.queries, d.q_hidden
         hd = H // d.q_heads
-        L = self.qf[0]
+        L = self.qf[0]                  # a cross-attention layer: i % cross_freq == 0
         with torch.cuda.device(self.dev):
-            h32, hhi, hlo = self.q0_32.clone(), self.q0_16.clone(), self.q0_lo.clone()
+            h32 = torch.empty(Q, H, dtype=F32, device=self.dev)
+            hhi, hlo = torch.empty(Q, H, dtype=F16, device=self.dev), torch.empty(Q, H, dtype=F16, device=self.dev)
+            dense.layernorm_x2(self.query_tokens, self.q_ln_w, self.q_ln_b, d.q_eps, hhi, hlo, h32)
             qkv, ahi, alo = self.q_qkv32[:Q], self.q_ao[:Q], self.q_ao_lo[:Q]
             self._gemm_x2(hhi, hlo, L["qkv_w"], L["qkv_wl"], L["qkv_b"], _lib.EPI_BIAS_F32, qkv)
-            self._attn32(qkv[:, 0:H], qkv[:, H : 2 * H], qkv[:, 2 * H : 3 * H], ahi, alo, 1, d.q_heads, Q, Q, hd, 1.0 / math.sqrt(hd))
+            dense.attention_f32(qkv[:, 0:H], qkv[:, H : 2 * H], qkv[:, 2 * H : 3 * H], 1, d.q_heads, Q, Q, hd, 1.0 / math.sqrt(hd), ahi, alo)
             self._gemm_x2_resid_ln(ahi, alo, L["so_w"], L["so_wl"], L["so_b"], h32, L["sln_w"], L["sln_b"], hhi, hlo, h32, d.q_eps)
-            self.f0_32, self.f0_hi, self.f0_lo = h32, hhi, hlo
-            self.f0_q = None
-            if L["cross"] >= 0:
-                self.f0_q = torch.empty(Q, H, dtype=F32, device=self.dev)
-                self._gemm_x2(hhi, hlo, L["cq_w"], L["cq_wl"], L["cq_b"], _lib.EPI_BIAS_F32, self.f0_q)
+            f0_q = torch.empty(Q, H, dtype=F32, device=self.dev)
+            self._gemm_x2(hhi, hlo, L["cq_w"], L["cq_wl"], L["cq_b"], _lib.EPI_BIAS_F32, f0_q)
             torch.cuda.synchronize()
-        self.f0_32x = self.f0_32.repeat(self.max_batch, 1)
-        self.f0_qx = self.f0_q.repeat(self.max_batch, 1) if self.f0_q is not None else None
-        self.fold0 = os.environ.get("VLFM_QFORMER_FOLD0", "1") != "0" and L["cross"] >= 0
+        self.f0_32x = h32.repeat(self.max_batch, 1)
+        self.f0_qx = f0_q.repeat(self.max_batch, 1)
 
-    def _qformer_layers_x2(self, h32, hhi, hlo, B, S, kv, T, text: bool, folded: bool = False) -> None:
-        """the same layers with x2 operands everywhere and float32 attention (modeling: Blip2QFormerLayer; float32 in the reference).
-        ``folded``: h32 / hhi / hlo already hold layer 0's self-attention block output (``_fold_layer0``)."""
+    def _qformer_layers(self, h32, hhi, hlo, B, S, kv, T, text: bool) -> None:
+        """The Q-Former layers (modeling: Blip2QFormerLayer; float32 in the reference) with x2 operands everywhere and float32
+        attention.  The image path (text=False) starts after layer 0's self-attention block, which _fold_layer0 computed: h32 holds
+        its output; the text path (query_length=0: no cross-attention) runs every layer."""
         d = self.d
         H = d.q_hidden
         hd = H // d.q_heads
@@ -374,19 +283,20 @@ class Blip2ITCEngine:
         qkv, qq, ahi, alo, fhi, flo = self.q_qkv32[:n], self.q_q32[:n], self.q_ao[:n], self.q_ao_lo[:n], self.q_f[:n], self.q_f_lo[:n]
         sc = 1.0 / math.sqrt(hd)
         for li, L in enumerate(self.qf):
-            skip = folded and li == 0
-            if not skip:
+            folded = not text and li == 0
+            if not folded:
                 self._gemm_x2(hhi, hlo, L["qkv_w"], L["qkv_wl"], L["qkv_b"], _lib.EPI_BIAS_F32, qkv)
-                self._attn32(qkv[:, 0:H], qkv[:, H : 2 * H], qkv[:, 2 * H : 3 * H], ahi, alo, B, d.q_heads, S, S, hd, sc)
+                dense.attention_f32(qkv[:, 0:H], qkv[:, H : 2 * H], qkv[:, 2 * H : 3 * H], B, d.q_heads, S, S, hd, sc, ahi, alo)
                 self._gemm_x2_resid_ln(ahi, alo, L["so_w"], L["so_wl"], L["so_b"], h32, L["sln_w"], L["sln_b"], hhi, hlo, h32, d.q_eps)
             if not text and L["cross"] >= 0:
                 j = L["cross"]
-                cq = qq
-                if skip:
+                if folded:
                     cq = self.f0_qx[:n]                  # constant: never written
                 else:
+                    cq = qq
                     self._gemm_x2(hhi, hlo, L["cq_w"], L["cq_wl"], L["cq_b"], _lib.EPI_BIAS_F32, qq)
-                self._attn32(cq, kv[:, j * 2 * H : j * 2 * H + H], kv[:, j * 2 * H + H : (j + 1) * 2 * H], ahi, alo, B, d.q_heads, S, T, hd, sc)
+                dense.attention_f32(cq, kv[:, j * 2 * H : j * 2 * H + H], kv[:, j * 2 * H + H : (j + 1) * 2 * H], B, d.q_heads, S, T, hd, sc,
+                                    ahi, alo)
                 self._gemm_x2_resid_ln(ahi, alo, L["co_w"], L["co_wl"], L["co_b"], h32, L["cln_w"], L["cln_b"], hhi, hlo, h32, d.q_eps)
             k1, k2, kl = ("it", "ot", "otln") if text else ("iq", "oq", "oqln")
             self._gemm_x2(hhi, hlo, L[k1 + "_w"], L[k1 + "_wl"], L[k1 + "_b"], _lib.EPI_BIAS_GELU_F16X2, fhi, flo)
@@ -402,18 +312,12 @@ class Blip2ITCEngine:
         S = len(ids)
         assert 1 <= S <= self.d.queries * self.max_batch and S <= 272
         emb = (self.word_emb[ids] + self.pos_emb[:S]).contiguous()
-        h32, h16 = self.q_h32[:S], self.q_h16[:S]
+        h32, hhi, hlo = self.q_h32[:S], self.q_h16[:S], self.q_h_lo[:S]
         with torch.cuda.device(self.dev):
             tp = torch.empty(1, d.proj, dtype=F32, device=self.dev)
-            if self.x2:
-                hlo = self.q_h_lo[:S]
-                self._ln_x2(emb, self.q_ln_w, self.q_ln_b, h16, hlo, h32, d.q_eps)
-                self._qformer_layers_x2(h32, h16, hlo, 1, S, None, 0, text=True)
-                self._gemm_x2(h16[:1], hlo[:1], self.tp_w, self.tp_wl, self.tp_b, _lib.EPI_BIAS_F32, tp)
-            else:
-                self._ln(emb, self.q_ln_w, self.q_ln_b, h16, h32, d.q_eps)
-                self._qformer_layers(h32, h16, 1, S, None, 0, text=True)
-                self._gemm(h16[:1], self.tp_w, self.tp_b, _lib.EPI_BIAS_F32, tp)
+            dense.layernorm_x2(emb, self.q_ln_w, self.q_ln_b, d.q_eps, hhi, hlo, h32)
+            self._qformer_layers(h32, hhi, hlo, 1, S, None, 0, text=True)
+            self._gemm_x2(hhi[:1], hlo[:1], self.tp_w, self.tp_wl, self.tp_b, _lib.EPI_BIAS_F32, tp)
         return torch.nn.functional.normalize(tp[0], dim=-1)
 
     def set_text(self, feat: torch.Tensor) -> None:
@@ -470,8 +374,3 @@ class Blip2ITCEngine:
                                               self.d.proj, P, _lib.stream_ptr())
         _lib.check(rc, "vlfm_itc_head_multi")
         return out[:B]
-
-    def launches_per_forward(self) -> int:
-        d = self.d
-        per_q = 7 + 0  # qkv, attn, dense, ln, inter, out, ln
-        return 2 + 1 + 1 + d.v_layers * 7 + 1 + 1 + d.q_layers * per_q + self.ncross * 4 + 1 + 1

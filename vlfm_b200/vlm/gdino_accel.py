@@ -15,13 +15,13 @@ import ctypes
 import torch
 
 from .. import _lib
+from .dense import cast_addpos_f16, cast_f16, gemm_f16, layernorm
+
+F16 = torch.float16
 
 
-def cast_f16(x: torch.Tensor) -> torch.Tensor:
-    """fp32 contiguous -> fp16 on the library's cast kernel."""
-    out = torch.empty(x.shape, dtype=torch.float16, device=x.device)
-    _lib.check(_lib.load().vlfm_cast_f32_f16(x.data_ptr(), out.data_ptr(), x.numel(), _lib.stream_ptr()), "vlfm_cast_f32_f16")
-    return out
+def _f16(x: torch.Tensor) -> torch.Tensor:
+    return torch.empty(x.shape, dtype=F16, device=x.device)
 
 
 class TcLinear(torch.nn.Module):
@@ -39,13 +39,9 @@ class TcLinear(torch.nn.Module):
             x2 = cast_f16(x2.float().contiguous())
         elif not x2.is_contiguous():
             x2 = x2.contiguous()
-        m = x2.shape[0]
-        out = torch.empty((m, self.out_features), dtype=torch.float32, device=x.device)
-        if m:
-            rc = _lib.load().vlfm_gemm_f16(x2.data_ptr(), self.w16.data_ptr(), _lib.ptr(self.b32), out.data_ptr(), m, self.out_features,
-                                          self.in_features, self.in_features, self.in_features, self.out_features, _lib.EPI_BIAS_F32,
-                                          _lib.stream_ptr())
-            _lib.check(rc, "vlfm_gemm_f16")
+        out = torch.empty((x2.shape[0], self.out_features), dtype=torch.float32, device=x.device)
+        if x2.shape[0]:                 # the GEMM refuses M = 0
+            gemm_f16(x2, self.w16, self.b32, _lib.EPI_BIAS_F32, out)
         return out.view(*shp[:-1], self.out_features)
 
 
@@ -97,17 +93,13 @@ class TcDeformAttn(torch.nn.Module):
 
     def sample(self, hidden: torch.Tensor, pos, enc, ref: torch.Tensor, shapes_list) -> torch.Tensor:
         """-> fp16 [B*Q, d] attention output before the output projection."""
-        from .dense import gemm_f16
-
-        lib = _lib.load()
         b, q, d = hidden.shape
         same = enc is None or enc is hidden
         x = hidden.contiguous()
-        xp16 = torch.empty((b * q, d), dtype=torch.float16, device=x.device)
-        x16 = torch.empty((b * q, d), dtype=torch.float16, device=x.device) if same else None
         p = None if pos is None else pos.expand_as(x).contiguous()
-        _lib.check(lib.vlfm_cast_addpos_f16(x.data_ptr(), _lib.ptr(p), _lib.ptr(x16), xp16.data_ptr(), x.numel(), _lib.stream_ptr()),
-                   "vlfm_cast_addpos_f16")
+        x = x.view(b * q, d)
+        x16 = _f16(x) if same else None
+        xp16 = cast_addpos_f16(x, p, x16)
         if not same:
             s = enc.shape[1]
             x16 = getattr(enc, "_vlfm_f16", None)      # the six decoder layers read the same encoder output
@@ -120,16 +112,14 @@ class TcDeformAttn(torch.nn.Module):
         offlog = gemm_f16(xp16, self.wc, self.bc, _lib.EPI_BIAS_F32)
         ref = ref.float().contiguous()
         out16 = torch.empty((b * q, d), dtype=torch.float16, device=x.device)
-        rc = lib.vlfm_msda_fused(value16.data_ptr(), offlog.data_ptr(), offlog.stride(0), self.logit_col, ref.data_ptr(), ref.shape[-1],
-                                 out16.data_ptr(), b, s, q, self.heads, self.levels, self.points,
-                                 ctypes.cast(_shapes(shapes_list), ctypes.c_void_p), _lib.stream_ptr())
+        rc = _lib.load().vlfm_msda_fused(value16.data_ptr(), offlog.data_ptr(), offlog.stride(0), self.logit_col, ref.data_ptr(),
+                                          ref.shape[-1], out16.data_ptr(), b, s, q, self.heads, self.levels, self.points,
+                                          ctypes.cast(_shapes(shapes_list), ctypes.c_void_p), _lib.stream_ptr())
         _lib.check(rc, "vlfm_msda_fused")
         return out16
 
     def forward(self, hidden_states, attention_mask=None, encoder_hidden_states=None, encoder_attention_mask=None, position_embeddings=None,
                 reference_points=None, spatial_shapes=None, spatial_shapes_list=None, level_start_index=None, output_attentions=False):
-        from .dense import gemm_f16
-
         b, q, d = hidden_states.shape
         out16 = self.sample(hidden_states, position_embeddings, encoder_hidden_states, reference_points, spatial_shapes_list)
         return gemm_f16(out16, self.wo, self.bo, _lib.EPI_BIAS_F32).view(b, q, d), None
@@ -153,16 +143,14 @@ class TcDeformableLayer(torch.nn.Module):
 
     def forward(self, hidden_states, attention_mask=None, position_embeddings=None, reference_points=None, spatial_shapes=None,
                 spatial_shapes_list=None, level_start_index=None, output_attentions=False):
-        from .dense import gemm_f16, layernorm
-
         b, s, d = hidden_states.shape
         x = hidden_states.reshape(b * s, d).clone()                                   # fp32 residual stream
         out16 = self.attn.sample(hidden_states, position_embeddings, None, reference_points, spatial_shapes_list)
         gemm_f16(out16, self.attn.wo, self.attn.bo, _lib.EPI_BIAS_RESID_F32, out=x)   # x += out_proj(attn)
-        x16, x32 = layernorm(x, self.g1, self.be1, self.eps1, want16=True, want32=True)
+        x16, x32 = layernorm(x, self.g1, self.be1, self.eps1, True, True)
         h16 = gemm_f16(x16, self.w1, self.b1, _lib.EPI_BIAS_RELU_F16)
         gemm_f16(h16, self.w2, self.b2, _lib.EPI_BIAS_RESID_F32, out=x32)             # x32 += fc2(relu(fc1(x)))
-        _, y = layernorm(x32, self.g2, self.be2, self.eps2, want16=False, want32=True)
+        _, y = layernorm(x32, self.g2, self.be2, self.eps2, out32=True)
         return y.view(b, s, d), None
 
 
@@ -216,14 +204,12 @@ class TcFusionLayer(torch.nn.Module):
         self.orig = [m]
 
     def forward(self, vision_features, text_features, attention_mask_vision=None, attention_mask_text=None):
-        from .dense import gemm_f16, layernorm
-
         b, nv, d = vision_features.shape
         t = text_features.shape[1]
         if t > self.MAX_TEXT:
             return self.orig[0](vision_features, text_features, attention_mask_vision, attention_mask_text)
-        v16, v32 = layernorm(vision_features.reshape(b * nv, d).contiguous(), self.gv, self.bev, self.epsv, want16=True, want32=True)
-        t16, t32 = layernorm(text_features.reshape(b * t, d).contiguous(), self.gt, self.bet, self.epst, want16=True, want32=True)
+        v16, v32 = layernorm(vision_features.reshape(b * nv, d).contiguous(), self.gv, self.bev, self.epsv, True, True)
+        t16, t32 = layernorm(text_features.reshape(b * t, d).contiguous(), self.gt, self.bet, self.epst, True, True)
         qv = gemm_f16(v16, self.wv, self.bv, _lib.EPI_BIAS_F16)            # [b*nv, 2e]: image queries | image values
         kt = gemm_f16(t16, self.wt, self.bt, _lib.EPI_BIAS_F16)            # [b*t, 2e]: text keys | text values
         e = self.e
@@ -262,35 +248,25 @@ class TcDecoderLayer(torch.nn.Module):
     def forward(self, hidden_states, position_embeddings=None, reference_points=None, spatial_shapes=None, spatial_shapes_list=None,
                 level_start_index=None, vision_encoder_hidden_states=None, vision_encoder_attention_mask=None,
                 text_encoder_hidden_states=None, text_encoder_attention_mask=None, self_attn_mask=None, output_attentions=False):
-        from .dense import gemm_f16, layernorm
-
         if self_attn_mask is not None or output_attentions:
             return self.orig[0](hidden_states, position_embeddings, reference_points, spatial_shapes, spatial_shapes_list, level_start_index,
                                 vision_encoder_hidden_states, vision_encoder_attention_mask, text_encoder_hidden_states,
                                 text_encoder_attention_mask, self_attn_mask, output_attentions)
-        lib = _lib.load()
         b, nq, d = hidden_states.shape
         t = text_encoder_hidden_states.shape[1]
         scale = 32 ** -0.5
         x = hidden_states.reshape(b * nq, d).clone()                              # fp32 residual stream
         pos = None if position_embeddings is None else position_embeddings.expand(b, nq, d).reshape(b * nq, d).contiguous()
-
-        def with_pos(x32, want_plain):
-            xp16 = torch.empty((b * nq, d), dtype=torch.float16, device=x32.device)
-            x16 = torch.empty((b * nq, d), dtype=torch.float16, device=x32.device) if want_plain else None
-            _lib.check(lib.vlfm_cast_addpos_f16(x32.data_ptr(), _lib.ptr(pos), _lib.ptr(x16), xp16.data_ptr(), x32.numel(), _lib.stream_ptr()),
-                       "vlfm_cast_addpos_f16")
-            return x16, xp16
-
         # ---- self-attention: q = k = x + pos, v = x
-        x16, xp16 = with_pos(x, True)
+        x16 = _f16(x)
+        xp16 = cast_addpos_f16(x, pos, x16)
         qk = gemm_f16(xp16, self.wqk, self.bqk, _lib.EPI_BIAS_F16)
         v = gemm_f16(x16, self.wv, self.bv, _lib.EPI_BIAS_F16)
         a = biattn_f16(qk[:, :d], qk[:, d:], v, b, self.heads, nq, nq, scale, head_dim=32)
         gemm_f16(a, self.wo, self.bo, _lib.EPI_BIAS_RESID_F32, out=x)
-        _, x = layernorm(x, self.g0, self.be0, self.eps[0], want16=False, want32=True)
+        _, x = layernorm(x, self.g0, self.be0, self.eps[0], out32=True)
         # ---- text cross-attention: q = x + pos, k = v = text
-        _, xp16 = with_pos(x, False)
+        xp16 = cast_addpos_f16(x, pos)
         q = gemm_f16(xp16, self.xq, self.xbq, _lib.EPI_BIAS_F16)
         txt = text_encoder_hidden_states
         t16 = getattr(txt, "_vlfm_f16", None)
@@ -300,15 +276,15 @@ class TcDecoderLayer(torch.nn.Module):
         kv = gemm_f16(t16, self.xkv, self.xbkv, _lib.EPI_BIAS_F16)
         a = biattn_f16(q, kv[:, :d], kv[:, d:], b, self.heads, nq, t, scale, head_dim=32)
         gemm_f16(a, self.xo, self.xbo, _lib.EPI_BIAS_RESID_F32, out=x)
-        _, x = layernorm(x, self.g1, self.be1, self.eps[1], want16=False, want32=True)
+        _, x = layernorm(x, self.g1, self.be1, self.eps[1], out32=True)
         # ---- deformable cross-attention over the image features
         out16 = self.deform.sample(x.view(b, nq, d), position_embeddings, vision_encoder_hidden_states, reference_points, spatial_shapes_list)
         gemm_f16(out16, self.deform.wo, self.deform.bo, _lib.EPI_BIAS_RESID_F32, out=x)
-        x16, x = layernorm(x, self.g2, self.be2, self.eps[2], want16=True, want32=True)
+        x16, x = layernorm(x, self.g2, self.be2, self.eps[2], True, True)
         # ---- FFN
         h16 = gemm_f16(x16, self.w1, self.b1, _lib.EPI_BIAS_RELU_F16)
         gemm_f16(h16, self.w2, self.b2, _lib.EPI_BIAS_RESID_F32, out=x)
-        _, y = layernorm(x, self.g3, self.be3, self.eps[3], want16=False, want32=True)
+        _, y = layernorm(x, self.g3, self.be3, self.eps[3], out32=True)
         return (y.view(b, nq, d),)
 
 

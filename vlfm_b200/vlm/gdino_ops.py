@@ -7,7 +7,7 @@ from typing import Optional
 import torch
 
 from .. import _lib
-from .dense import gemm_f16, layernorm as _layernorm
+from .dense import cast_f16, gemm_f16, layernorm as _layernorm
 
 F16, F32 = torch.float16, torch.float32
 
@@ -23,11 +23,7 @@ class LibOps:
         return w
 
     def to_operand(self, x: torch.Tensor) -> torch.Tensor:
-        if x.dtype == F16:
-            return x
-        out = torch.empty(x.shape, dtype=F16, device=x.device)
-        _lib.check(self.lib.vlfm_cast_f32_f16(x.data_ptr(), out.data_ptr(), x.numel(), _lib.stream_ptr()), "vlfm_cast_f32_f16")
-        return out
+        return x if x.dtype == F16 else cast_f16(x)
 
     def linear_operand(self, a16: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.Tensor]) -> torch.Tensor:
         return gemm_f16(a16, w16, bias, _lib.EPI_BIAS_F32)
@@ -37,7 +33,7 @@ class LibOps:
         return gemm_f16(self.to_operand(x.contiguous()), w16, bias, _lib.EPI_BIAS_RELU_F16 if relu else _lib.EPI_BIAS_F32)
 
     def layernorm(self, x: torch.Tensor, g: torch.Tensor, b: torch.Tensor, eps: float) -> torch.Tensor:
-        return _layernorm(x, g, b, eps, want16=False, want32=True)[1]
+        return _layernorm(x, g, b, eps, out32=True)[1]
 
     # ---- neck
     def im2col3x3s2(self, rows: torch.Tensor, B: int, h: int, w: int) -> torch.Tensor:

@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from .. import _lib
+from .dense import attention_f16, gemm_f16, gemm_f16_resid_ln, layernorm
 from .preprocess import bilinear_tables
 from .sam_config import SamDims
 
@@ -74,30 +75,8 @@ class MobileSamEngine:
         self._dec: Dict[int, Dict[str, torch.Tensor]] = {}
 
     # ---------------------------------------------------------------------------------------------------- primitives
-    def _gemm(self, a, wname, epi, out, rows=None, bias=True):
-        W = self.w[wname + ".w"] if not wname.endswith(".w") else self.w[wname]
-        b = self.w.get(wname + ".b") if bias else None
-        M = rows if rows is not None else a.shape[0]
-        rc = self.lib.vlfm_gemm_f16(a.data_ptr(), W.data_ptr(), _lib.ptr(b), out.data_ptr(), M, W.shape[0], W.shape[1], a.stride(0),
-                                    W.stride(0), out.stride(0), epi, _lib.stream_ptr())
-        _lib.check(rc, f"vlfm_gemm_f16({wname})")
-
-    def _gemm_resid_ln(self, a, wname, x, ln, out16, out32, rows, eps=1e-5):
-        W, b = self.w[wname + ".w"], self.w[wname + ".b"]
-        g, be = self.w[ln + ".w"], self.w[ln + ".b"]
-        rc = self.lib.vlfm_gemm_f16_resid_ln(a.data_ptr(), W.data_ptr(), b.data_ptr(), x.data_ptr(), rows, W.shape[0], W.shape[1],
-                                             a.stride(0), W.stride(0), x.stride(0), g.data_ptr(), be.data_ptr(), _lib.ptr(out16),
-                                             out16.stride(0) if out16 is not None else 0, _lib.ptr(out32),
-                                             out32.stride(0) if out32 is not None else 0, eps, None, 0, _lib.stream_ptr())
-        _lib.check(rc, f"vlfm_gemm_f16_resid_ln({wname})")
-
-    def _ln(self, x, ln, out16, out32, eps, rows=None):
-        g, be = self.w[ln + ".w"], self.w[ln + ".b"]
-        rc = self.lib.vlfm_layernorm(x.data_ptr(), g.data_ptr(), be.data_ptr(), _lib.ptr(out16), _lib.ptr(out32),
-                                     rows if rows is not None else x.shape[0], x.shape[1], x.stride(0),
-                                     out16.stride(0) if out16 is not None else 0, out32.stride(0) if out32 is not None else 0, eps,
-                                     _lib.stream_ptr())
-        _lib.check(rc, "vlfm_layernorm")
+    def _wb(self, name):    # (weight, bias or None) of a GEMM; (gamma, beta) of a LayerNorm
+        return self.w[name + ".w"], self.w.get(name + ".b")
 
     def _dw(self, x, x_f32, name, out, out_f32, B, H, W, C, stride, gelu):
         rc = self.lib.vlfm_sam_dwconv3x3(x.data_ptr(), x_f32, self.w[name + ".w"].data_ptr(), self.w[name + ".b"].data_ptr(), out.data_ptr(),
@@ -171,12 +150,12 @@ class MobileSamEngine:
         col = v(A, B * h1 * h1, self.w["stem0.w"].shape[1])
         self._im2col(x0, col, B, S, S, 3, 2)
         s0 = v(Bb, B * h1 * h1, d.stem_mid)
-        self._gemm(col, "stem0", _lib.EPI_BIAS_GELU_F16, s0)
+        gemm_f16(col, *self._wb("stem0"), _lib.EPI_BIAS_GELU_F16, s0)
         n0 = B * r[0] * r[0]
         col = v(A, n0, self.w["stem1.w"].shape[1])
         self._im2col(s0, col, B, h1, h1, d.stem_mid, 2)
         x32, y32, z32, x16 = v(bf["x32"], n0, E[0]), v(bf["y32"], n0, E[0]), v(bf["z32"], n0, E[0]), v(bf["x16"], n0, E[0])
-        self._gemm(col, "stem1", _lib.EPI_BIAS_F32, x32)
+        gemm_f16(col, *self._wb("stem1"), _lib.EPI_BIAS_F32, x32)
         self._add_act(x32, None, None, x16, x32.numel(), 0)
         for s in range(len(E)):
             C, R = E[s], r[s]
@@ -187,46 +166,46 @@ class MobileSamEngine:
                 if s == 0:      # MBConv: 1x1 + GELU, dw3x3 + GELU, 1x1, + shortcut, GELU
                     hid = C * d.mbconv_ratio
                     t1, t2 = v(A, n, hid), v(Bb, n, hid)
-                    self._gemm(x16, p + "conv1", _lib.EPI_BIAS_GELU_F16, t1)
+                    gemm_f16(x16, *self._wb(p + "conv1"), _lib.EPI_BIAS_GELU_F16, t1)
                     self._dw(t1, 0, p + "conv2", t2, 0, B, R, R, hid, 1, 1)
-                    self._gemm(t2, p + "conv3", _lib.EPI_BIAS_F32, y32)
+                    gemm_f16(t2, *self._wb(p + "conv3"), _lib.EPI_BIAS_F32, y32)
                     self._add_act(y32, x32, x32, x16, n * C, 1)
                     continue
                 heads, ws = d.heads[s], d.windows[s]
                 xn, qkv, ao, hh = v(A, n, C), v(Bb, n, 3 * C), v(A[n * C:], n, C), v(Bb, n, 4 * C)
-                self._ln(x32, p + "ln1", xn, None, 1e-5)
-                self._gemm(xn, p + "qkv", _lib.EPI_BIAS_F16, qkv)
+                layernorm(x32, *self._wb(p + "ln1"), 1e-5, xn)
+                gemm_f16(xn, *self._wb(p + "qkv"), _lib.EPI_BIAS_F16, qkv)
                 rc = self.lib.vlfm_sam_window_attention(qkv.data_ptr(), self.w[p + "pad_qkv"].data_ptr(), self.w[p + "bias"].data_ptr(),
                                                         ao.data_ptr(), B, R, R, C, heads, ws, float((C // heads) ** -0.5), _lib.stream_ptr())
                 _lib.check(rc, "vlfm_sam_window_attention")
-                self._gemm(ao, p + "proj", _lib.EPI_BIAS_RESID_F32, x32)      # K = C <= 320: one K split, no atomics
+                gemm_f16(ao, *self._wb(p + "proj"), _lib.EPI_BIAS_RESID_F32, x32)      # K = C <= 320: one K split, no atomics
                 self._dw(x32, 1, p + "local", z32, 1, B, R, R, C, 1, 0)
-                self._ln(z32, p + "ln2", xn, None, 1e-5)
-                self._gemm(xn, p + "fc1", _lib.EPI_BIAS_GELU_F16, hh)
-                self._gemm(hh, p + "fc2", _lib.EPI_BIAS_F32, y32)
+                layernorm(z32, *self._wb(p + "ln2"), 1e-5, xn)
+                gemm_f16(xn, *self._wb(p + "fc1"), _lib.EPI_BIAS_GELU_F16, hh)
+                gemm_f16(hh, *self._wb(p + "fc2"), _lib.EPI_BIAS_F32, y32)
                 self._add_act(y32, z32, x32, x16, n * C, 0)
             if s + 1 < len(E):   # PatchMerging: 1x1 + GELU, dw3x3 (stride) + GELU, 1x1
                 Co, st = E[s + 1], d.merge_stride(s)
                 Ro = r[s + 1]
                 no = B * Ro * Ro
                 t1, t2 = v(A, n, Co), v(Bb, no, Co)
-                self._gemm(x16, f"l{s}.down.conv1", _lib.EPI_BIAS_GELU_F16, t1)
+                gemm_f16(x16, *self._wb(f"l{s}.down.conv1"), _lib.EPI_BIAS_GELU_F16, t1)
                 self._dw(t1, 0, f"l{s}.down.conv2", t2, 0, B, R, R, Co, st, 1)
                 x32n = v(bf["x32"], no, Co)
-                self._gemm(t2, f"l{s}.down.conv3", _lib.EPI_BIAS_F32, x32n)
+                gemm_f16(t2, *self._wb(f"l{s}.down.conv3"), _lib.EPI_BIAS_F32, x32n)
         # neck: 1x1 (no bias) -> LayerNorm2d -> 3x3 (no bias) -> LayerNorm2d
         R, P = r[-1], d.prompt_dim
         n = B * R * R
         x16 = v(bf["x16"], n, E[-1])
         t32 = v(bf["y32"], n, P)
-        self._gemm(x16, "neck0.w", _lib.EPI_BIAS_F32, t32, bias=False)
+        gemm_f16(x16, *self._wb("neck0"), _lib.EPI_BIAS_F32, t32)
         t16 = v(Bb, n, P)
-        self._ln(t32, "neck1", t16, None, 1e-6)
+        layernorm(t32, *self._wb("neck1"), 1e-6, t16)
         col = v(A, n, self.w["neck2.w"].shape[1])
         self._im2col(t16, col, B, R, R, P, 1)
-        self._gemm(col, "neck2.w", _lib.EPI_BIAS_F32, t32, bias=False)
+        gemm_f16(col, *self._wb("neck2"), _lib.EPI_BIAS_F32, t32)
         out = self.emb[:B].view(n, P)
-        self._ln(t32, "neck3", None, out, 1e-6)
+        layernorm(t32, *self._wb("neck3"), 1e-6, out32=out)
         self.frames = B
         self.generation += 1
         return self.emb[:B]
@@ -263,19 +242,14 @@ class MobileSamEngine:
         d, P = self.d, self.d.prompt_dim
         tq, to = bf["tq"][:, : P // 2], bf["to"][:, : P // 2]
         tk, tv = bf["iq"][: M * HW], bf["iv"][: M * HW]
-        self._gemm(qsrc, p + ".q", _lib.EPI_BIAS_F16, tq, rows=T)
-        self._gemm(ksrc, p + ".k", _lib.EPI_BIAS_F16, tk)
-        self._gemm(vsrc, p + ".v", _lib.EPI_BIAS_F16, tv)
+        gemm_f16(qsrc, *self._wb(p + ".q"), _lib.EPI_BIAS_F16, tq, rows=T)
+        gemm_f16(ksrc, *self._wb(p + ".k"), _lib.EPI_BIAS_F16, tk)
+        gemm_f16(vsrc, *self._wb(p + ".v"), _lib.EPI_BIAS_F16, tv)
         rc = self.lib.vlfm_sam_t2i_attention(tq.data_ptr(), tk.data_ptr(), tv.data_ptr(), to.data_ptr(), M, d.dec_heads, 7, HW, tq.stride(0),
                                              tk.stride(0), tv.stride(0), to.stride(0), float((P // 2 // d.dec_heads) ** -0.5),
                                              bf["part"].data_ptr(), bf["part"].numel(), _lib.stream_ptr())
         _lib.check(rc, "vlfm_sam_t2i_attention")
         return to
-
-    def _attn_f16(self, q, k, v, o, B, Nq, Nk, hd, scale):
-        rc = self.lib.vlfm_attention_f16(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), B, self.d.dec_heads, Nq, Nk, hd,
-                                         q.stride(0), k.stride(0), v.stride(0), o.stride(0), scale, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_attention_f16")
 
     @torch.inference_mode()
     def decode(self, boxes: torch.Tensor, frame_idx: torch.Tensor, hw: Tuple[int, int], out: torch.Tensor = None,
@@ -317,51 +291,51 @@ class MobileSamEngine:
             else:
                 self._add_pe(qs, tok0, q16, qp16, T, T)
                 src_qk = qp16
-            self._gemm(src_qk, p + ".self.q", _lib.EPI_BIAS_F16, bf["tq"], rows=T)
-            self._gemm(src_qk, p + ".self.k", _lib.EPI_BIAS_F16, bf["tk"], rows=T)
-            self._gemm(q16, p + ".self.v", _lib.EPI_BIAS_F16, bf["tv"], rows=T)
+            gemm_f16(src_qk, *self._wb(p + ".self.q"), _lib.EPI_BIAS_F16, bf["tq"], rows=T)
+            gemm_f16(src_qk, *self._wb(p + ".self.k"), _lib.EPI_BIAS_F16, bf["tk"], rows=T)
+            gemm_f16(q16, *self._wb(p + ".self.v"), _lib.EPI_BIAS_F16, bf["tv"], rows=T)
             for g0 in range(0, M, SELF_ATTN_GROUP):
                 gb = min(SELF_ATTN_GROUP, M - g0)
                 r0 = 7 * g0
-                self._attn_f16(bf["tq"][r0:], bf["tk"][r0:], bf["tv"][r0:], bf["to"][r0:], gb, 7, 7, hd_s, float(hd_s ** -0.5))
+                attention_f16(bf["tq"][r0:], bf["tk"][r0:], bf["tv"][r0:], gb, d.dec_heads, 7, 7, hd_s, float(hd_s ** -0.5), bf["to"][r0:])
             if i == 0:
                 qs.zero_()
-            self._gemm_resid_ln(bf["to"], p + ".self.o", qs, f"{p}.norm1", None, qs, T)
+            gemm_f16_resid_ln(bf["to"], *self._wb(p + ".self.o"), qs, *self._wb(f"{p}.norm1"), 1e-5, out32=qs, rows=T)
             # token -> image
             self._add_pe(qs, tok0, None, qp16, T, T)
             self._add_pe(keys, self.dense_pe, k16, kp16, M * HW, HW)
             to = self._t2i(p + ".t2i", bf, M, HW, qp16, kp16, k16, T)
-            self._gemm_resid_ln(to, p + ".t2i.o", qs, f"{p}.norm2", q16, qs, T)
+            gemm_f16_resid_ln(to, *self._wb(p + ".t2i.o"), qs, *self._wb(f"{p}.norm2"), 1e-5, q16, qs, rows=T)
             # MLP
-            self._gemm(q16, p + ".mlp1", _lib.EPI_BIAS_RELU_F16, bf["h16"], rows=T)
-            self._gemm_resid_ln(bf["h16"], p + ".mlp2", qs, f"{p}.norm3", None, qs, T)
+            gemm_f16(q16, *self._wb(p + ".mlp1"), _lib.EPI_BIAS_RELU_F16, bf["h16"], rows=T)
+            gemm_f16_resid_ln(bf["h16"], *self._wb(p + ".mlp2"), qs, *self._wb(f"{p}.norm3"), 1e-5, out32=qs, rows=T)
             # image -> token (keys unchanged since the token -> image step: kp16 still holds keys + pe)
             self._add_pe(qs, tok0, q16, qp16, T, T)
             iq, ik, iv, io = bf["iq"][: M * HW], bf["tk"][:, : P // 2], bf["tv"][:, : P // 2], bf["iv"][: M * HW]
-            self._gemm(kp16, p + ".i2t.q", _lib.EPI_BIAS_F16, iq)
-            self._gemm(qp16, p + ".i2t.k", _lib.EPI_BIAS_F16, ik, rows=T)
-            self._gemm(q16, p + ".i2t.v", _lib.EPI_BIAS_F16, iv, rows=T)
+            gemm_f16(kp16, *self._wb(p + ".i2t.q"), _lib.EPI_BIAS_F16, iq)
+            gemm_f16(qp16, *self._wb(p + ".i2t.k"), _lib.EPI_BIAS_F16, ik, rows=T)
+            gemm_f16(q16, *self._wb(p + ".i2t.v"), _lib.EPI_BIAS_F16, iv, rows=T)
             hd_c = P // 2 // d.dec_heads
-            self._attn_f16(iq, ik, iv, io, M, HW, 7, hd_c, float(hd_c ** -0.5))
-            self._gemm_resid_ln(io, p + ".i2t.o", keys, f"{p}.norm4", None, keys, M * HW)
+            attention_f16(iq, ik, iv, M, d.dec_heads, HW, 7, hd_c, float(hd_c ** -0.5), io)
+            gemm_f16_resid_ln(io, *self._wb(p + ".i2t.o"), keys, *self._wb(f"{p}.norm4"), 1e-5, out32=keys, rows=M * HW)
         # final token -> image attention
         self._add_pe(qs, tok0, None, qp16, T, T)
         self._add_pe(keys, self.dense_pe, k16, kp16, M * HW, HW)
         to = self._t2i("final", bf, M, HW, qp16, kp16, k16, T)
-        self._gemm_resid_ln(to, "final.o", qs, "norm_final", q16, qs, T)
+        gemm_f16_resid_ln(to, *self._wb("final.o"), qs, *self._wb("norm_final"), 1e-5, q16, qs, rows=T)
         # upscaling: ConvT 2x2 s2 -> LayerNorm2d -> GELU -> ConvT 2x2 s2 -> GELU, then the mask-0 hypernetwork dot product
         u1 = bf["u1"][: M * HW]
-        self._gemm(k16, "up1", _lib.EPI_BIAS_F32, u1)
+        gemm_f16(k16, *self._wb("up1"), _lib.EPI_BIAS_F32, u1)
         u1s, u1n, u16, u2 = bf["u1s"][: 4 * M * HW], bf["u1n"][: 4 * M * HW], bf["u16"][: 4 * M * HW], bf["u2"][: 4 * M * HW]
         rc = self.lib.vlfm_sam_pixel_shuffle2(u1.data_ptr(), u1s.data_ptr(), M, e, e, P // 4, st)
         _lib.check(rc, "vlfm_sam_pixel_shuffle2")
-        self._ln(u1s, "up_ln", None, u1n, 1e-6)
+        layernorm(u1s, *self._wb("up_ln"), 1e-6, out32=u1n)
         self._add_act(u1n, None, None, u16, u1n.numel(), 1)
-        self._gemm(u16, "up2", _lib.EPI_BIAS_F32, u2)
+        gemm_f16(u16, *self._wb("up2"), _lib.EPI_BIAS_F32, u2)
         tok1 = q16[1:].as_strided((Mp, P), (7 * P, 1))
-        self._gemm(tok1, "hyper0", _lib.EPI_BIAS_RELU_F16, bf["hy1"])
-        self._gemm(bf["hy1"], "hyper1", _lib.EPI_BIAS_RELU_F16, bf["hy2"])
-        self._gemm(bf["hy2"], "hyper2", _lib.EPI_BIAS_F32, bf["hyper"])
+        gemm_f16(tok1, *self._wb("hyper0"), _lib.EPI_BIAS_RELU_F16, bf["hy1"])
+        gemm_f16(bf["hy1"], *self._wb("hyper1"), _lib.EPI_BIAS_RELU_F16, bf["hy2"])
+        gemm_f16(bf["hy2"], *self._wb("hyper2"), _lib.EPI_BIAS_F32, bf["hyper"])
         L = 4 * e
         low = bf["low"][:M]
         rc = self.lib.vlfm_sam_mask_logits(u2.data_ptr(), bf["hyper"].data_ptr(), low.data_ptr(), M, 2 * e, 2 * e, P // 8, st)

@@ -17,6 +17,7 @@ from typing import Dict, List, Sequence, Tuple
 import torch
 
 from .. import _lib
+from .dense import gemm_f16, layernorm
 
 F16, F32 = torch.float16, torch.float32
 IMAGENET_MEAN = (0.485, 0.456, 0.406)
@@ -67,19 +68,6 @@ class SwinBackboneEngine:
             self.stages.append(st)
         self._bufs: Dict[Tuple[int, int, int], Dict[str, torch.Tensor]] = {}
 
-    # ---- primitives
-    def _gemm(self, a, w, bias, epi, out):
-        rc = self.lib.vlfm_gemm_f16(a.data_ptr(), w.data_ptr(), _lib.ptr(bias), out.data_ptr(), a.shape[0], w.shape[0], a.shape[1],
-                                    a.stride(0), w.stride(0), out.stride(0), epi, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_gemm_f16")
-
-    def _ln(self, x, wb, out16, out32):
-        rows, D = x.shape
-        rc = self.lib.vlfm_layernorm(x.data_ptr(), wb[0].data_ptr(), wb[1].data_ptr(), _lib.ptr(out16), _lib.ptr(out32), rows, D,
-                                     x.stride(0), out16.stride(0) if out16 is not None else 0,
-                                     out32.stride(0) if out32 is not None else 0, self.eps, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_layernorm")
-
     def _buffers(self, B: int, H: int, W: int) -> Dict[str, torch.Tensor]:
         key = (B, H, W)
         if key not in self._bufs:
@@ -111,8 +99,8 @@ class SwinBackboneEngine:
             n = B * h * w
             flat = lambda t, rows, cols: t.view(-1)[: rows * cols].view(rows, cols)
             x = flat(bufs["x"], n, C)
-            self._gemm(bufs["col"], self.pe_w, self.pe_b, _lib.EPI_BIAS_F32, x)
-            self._ln(x, self.pe_ln, None, x)
+            gemm_f16(bufs["col"], self.pe_w, self.pe_b, _lib.EPI_BIAS_F32, x)
+            layernorm(x, *self.pe_ln, self.eps, out32=x)
             feats: List[torch.Tensor] = []
             cur, other = "x", "x2"
             for s, stage in enumerate(self.stages):
@@ -125,18 +113,18 @@ class SwinBackboneEngine:
                 x = flat(bufs[cur], n, C)
                 xn, qkv, ao, hh = flat(bufs["xn"], n, C), flat(bufs["qkv"], n, 3 * C), flat(bufs["ao"], n, C), flat(bufs["h"], n, 4 * C)
                 for blk in stage["blocks"]:
-                    self._ln(x, blk["ln1"], xn, None)
-                    self._gemm(xn, blk["qkv_w"], blk["qkv_b"], _lib.EPI_BIAS_F16, qkv)
+                    layernorm(x, *blk["ln1"], self.eps, xn)
+                    gemm_f16(xn, blk["qkv_w"], blk["qkv_b"], _lib.EPI_BIAS_F16, qkv)
                     rc = lib.vlfm_swin_window_attention(qkv.data_ptr(), blk["qkv_b"].data_ptr(), blk["rel"].data_ptr(), ao.data_ptr(),
                                                         B, h, w, C, self.heads[s], blk["shift"], st)
                     _lib.check(rc, "vlfm_swin_window_attention")
-                    self._gemm(ao, blk["proj_w"], blk["proj_b"], _lib.EPI_BIAS_RESID_F32, x)
-                    self._ln(x, blk["ln2"], xn, None)
-                    self._gemm(xn, blk["fc1_w"], blk["fc1_b"], _lib.EPI_BIAS_GELU_F16, hh)
-                    self._gemm(hh, blk["fc2_w"], blk["fc2_b"], _lib.EPI_BIAS_RESID_F32, x)
+                    gemm_f16(ao, blk["proj_w"], blk["proj_b"], _lib.EPI_BIAS_RESID_F32, x)
+                    layernorm(x, *blk["ln2"], self.eps, xn)
+                    gemm_f16(xn, blk["fc1_w"], blk["fc1_b"], _lib.EPI_BIAS_GELU_F16, hh)
+                    gemm_f16(hh, blk["fc2_w"], blk["fc2_b"], _lib.EPI_BIAS_RESID_F32, x)
                 if "out_ln" in stage:
                     o = torch.empty(n, C, dtype=F32, device=self.dev)
-                    self._ln(x, stage["out_ln"], None, o)
+                    layernorm(x, *stage["out_ln"], self.eps, out32=o)
                     feats.append((o, h, w) if rows else o.view(B, h, w, C).permute(0, 3, 1, 2).contiguous())
                 if "merge_w" in stage:
                     h2, w2 = (h + 1) // 2, (w + 1) // 2
@@ -145,9 +133,9 @@ class SwinBackboneEngine:
                     rc = lib.vlfm_swin_patch_merge(x.data_ptr(), mg.data_ptr(), B, h, w, C, st)
                     _lib.check(rc, "vlfm_swin_patch_merge")
                     mn = flat(bufs["xn"], n2, 4 * C)
-                    self._ln(mg, stage["merge_ln"], mn, None)
+                    layernorm(mg, *stage["merge_ln"], self.eps, mn)
                     nx = flat(bufs[other], n2, 2 * C)
-                    self._gemm(mn, stage["merge_w"], None, _lib.EPI_BIAS_F32, nx)
+                    gemm_f16(mn, stage["merge_w"], None, _lib.EPI_BIAS_F32, nx)
                     cur, other = other, cur
                     h, w, C = h2, w2, 2 * C
         return feats
