@@ -245,18 +245,14 @@ int vlfm_value_cone_template(double fov, double max_depth, int ppm, double min_c
                              size_t scratch_bytes, void* stream);
 
 /* ------------------------------------- GroundingDINO feature enhancer / decoder ---- */
-/* Multi-scale deformable attention sampling (replaces groundingdino's third-party ms_deform_attn_cuda.cu, reached from
- * vlfm/vlm/grounding_dino.py:61-67).  d_value [B,S,heads,hd] fp32 or fp16 (S = sum H_l*W_l, levels concatenated),
- * d_loc [B,Q,heads,levels,points,2] fp32 normalised (x,y), d_attw [B,Q,heads,levels,points] fp32 (already soft-maxed)
- * -> d_out [B,Q,heads*hd] fp32.  Bilinear taps with zero padding, align_corners=False.  h_shapes_hw: HOST int32
- * [levels*2] = (H_l, W_l). */
-int vlfm_msda_forward(const void* d_value, int value_is_f16, const float* d_loc, const float* d_attw, float* d_out, int B, int S,
-                      int Q, int heads, int hd, int levels, int points, const int32_t* h_shapes_hw, void* stream);
-/* Fused form used by the deformable layers: softmax over the levels*points logits, sampling-location arithmetic
+/* Multi-scale deformable attention (replaces groundingdino's third-party ms_deform_attn_cuda.cu, reached from
+ * vlfm/vlm/grounding_dino.py:61-67): softmax over the levels*points logits, sampling-location arithmetic
  * (MSDeformAttn.forward: loc = ref + off / (W_l, H_l) for 2-d reference points, ref_xy + off / points * ref_wh * 0.5 for
- * 4-d boxes) and the bilinear gather in one kernel.  d_value16 [B,S,heads,32] fp16; d_offlog [B*Q, ld] fp32 rows holding
+ * 4-d boxes) and the bilinear gather (zero padding, align_corners=False) in one kernel.  d_value16 [B,S,heads,32] fp16
+ * (S = sum H_l*W_l, levels concatenated); d_offlog [B*Q, ld] fp32 rows holding
  * the sampling-offset projection at column 0 (heads*levels*points*2) and the attention logits at column `logit_col`
- * (heads*levels*points); d_ref [B,Q,levels,ref_dim] fp32; d_out16 [B*Q, heads*32] fp16.  head_dim 32, levels*points <= 16. */
+ * (heads*levels*points); d_ref [B,Q,levels,ref_dim] fp32; d_out16 [B*Q, heads*32] fp16.  head_dim 32, levels*points <= 16.
+ * h_shapes_hw: HOST int32 [levels*2] = (H_l, W_l). */
 int vlfm_msda_fused(const void* d_value16, const float* d_offlog, int ld, int logit_col, const float* d_ref, int ref_dim,
                     void* d_out16, int B, int S, int Q, int heads, int levels, int points, const int32_t* h_shapes_hw,
                     void* stream);

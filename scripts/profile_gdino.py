@@ -22,14 +22,14 @@ def hook(name):
     def post(m, a, o):
         e = torch.cuda.Event(enable_timing=True); e.record(); times[name][-1][1] = e
     return pre, post
-mods = {"text_backbone": gd.model.model.text_backbone, "encoder": gd.model.model.encoder, "decoder": gd.model.model.decoder,
-        "backbone(conv_encoder+pos)": gd.model.model.backbone}
-for i, l in enumerate(gd.model.model.encoder.layers[:1]):
-    mods["enc0.fusion"] = l.fusion_layer; mods["enc0.text_enh"] = l.text_enhancer_layer; mods["enc0.deform"] = l.deformable_layer
-for i, l in enumerate(gd.model.model.decoder.layers[:1]):
-    mods["dec0"] = l
+# GdinoForward sequences the encoder / decoder stacks itself: the per-layer modules are what is called.  Hooks fire on eager
+# forwards only (B above VLFM_GDINO_GRAPH_MAX_BATCH, or VLFM_GDINO_GRAPH=0).
+mods = []
+for l in gd.model.model.encoder.layers:
+    mods += [("enc.fusion", l.fusion_layer), ("enc.text_enh", l.text_enhancer_layer), ("enc.deform", l.deformable_layer)]
+mods += [("dec.layer", l) for l in gd.model.model.decoder.layers]
 hs = []
-for n, m in mods.items():
+for n, m in mods:
     pre, post = hook(n)
     hs.append(m.register_forward_pre_hook(pre)); hs.append(m.register_forward_hook(post))
 e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True); e2 = torch.cuda.Event(enable_timing=True)

@@ -6,7 +6,6 @@ from vlfm_b200.mapping.obstacle_map import ObstacleMap
 from vlfm_b200.mapping.value_map import build_cone_template
 from vlfm_b200.utils.synthetic import focal_from_hfov, trajectory
 from vlfm_b200.vlm.dense import cast_f16
-from vlfm_b200.vlm.gdino_accel import TcMSDA
 from vlfm_b200 import _lib
 import ctypes
 
@@ -22,10 +21,7 @@ shapes = [(15, 20), (8, 10), (4, 5), (2, 3)]
 b, heads, hd, q, pts = 2, 8, 32, 77, 4
 s = sum(h * w for h, w in shapes)
 value = torch.randn(b, s, heads, hd, device="cuda")
-loc = torch.rand(b, q, heads, 4, pts, 2, device="cuda") * 1.3 - 0.15
-attw = torch.softmax(torch.randn(b, q, heads, 16, device="cuda"), -1).view(b, q, heads, 4, pts)
-o = TcMSDA()(value, None, shapes, None, loc, attw)
-# fused kernel
+# fused deformable attention
 offlog = torch.randn(b * q, 384, device="cuda")
 ref = torch.rand(b, q, 4, 2, device="cuda")
 out16 = torch.empty(b * q, 256, dtype=torch.float16, device="cuda")
@@ -41,4 +37,4 @@ _lib.check(rc, "msda_fused4")
 x = torch.randn(1003, device="cuda")
 h = cast_f16(x)
 torch.cuda.synchronize()
-print("ok", float(o.abs().sum()), float(out16.float().abs().sum()), float(h.float().sum()))
+print("ok", float(out16.float().abs().sum()), float(h.float().sum()))

@@ -1,62 +1,21 @@
-"""Host-side pieces of the GroundingDINO acceleration layer that need no GPU: the torch proxy that serves HF's host-list ->
-device-tensor constructions from a cache (what makes the module graph CUDA-graph capturable) and the per-caption text cache."""
+"""Host-side pieces of the GroundingDINO acceleration layer that need no GPU: which HF modules ``accelerate`` replaces, and that
+it leaves transformers' modelling code as it found it."""
 import torch
 
 from vlfm_b200.vlm import gdino_accel as ga
 
 
-def test_torch_proxy_forwards_and_caches_only_cuda_lists():
-    p = ga._TorchProxy(torch)
-    assert p.cat is torch.cat and p.nn is torch.nn and p.float32 is torch.float32
-    a = p.as_tensor([[1, 2], [3, 4]], dtype=torch.long, device="cpu")          # host target: never cached
-    b = p.as_tensor([[1, 2], [3, 4]], dtype=torch.long, device="cpu")
-    assert a is not b and torch.equal(a, b) and not p._cache
-    t = torch.ones(3)
-    assert p.as_tensor(t) is t                                                   # tensors pass straight through
-    calls = []
-
-    def fake_as_tensor(data, *args, **kw):                                       # stand-in for a CUDA construction
-        calls.append(data)
-        return torch.as_tensor(data, dtype=kw.get("dtype"))
-
-    fake_as_tensor.__name__ = "as_tensor"
-    r1 = p._cached(fake_as_tensor, [(60, 80), (30, 40)], (), {"dtype": torch.long, "device": "cuda:0"})
-    r2 = p._cached(fake_as_tensor, [(60, 80), (30, 40)], (), {"dtype": torch.long, "device": "cuda:0"})
-    r3 = p._cached(fake_as_tensor, [(60, 80), (15, 20)], (), {"dtype": torch.long, "device": "cuda:0"})
-    assert r1 is r2 and r3 is not r1 and len(calls) == 2
-
-
-def test_cached_text_backbone_runs_once_per_key():
-    class Inner(torch.nn.Module):
-        def __init__(self):
-            super().__init__()
-            self.n = 0
-
-        def forward(self, ids):
-            self.n += 1
-            return ids.float() * self.n
-
-    tb = ga.CachedTextBackbone(Inner(), max_entries=2)
-    ids = torch.tensor([[1, 2, 3]])
-    assert torch.equal(tb(ids), ids.float()) and tb.inner.n == 1                  # no key: plain call
-    tb.key = ((1, 2, 3), 1)
-    a, b = tb(ids), tb(ids)
-    assert a is b and tb.inner.n == 2
-    tb.key = ((4,), 1); tb(ids)
-    tb.key = ((5,), 1); tb(ids)                                                   # evicts the oldest entry
-    assert len(tb.cache) == 2 and ((1, 2, 3), 1) not in tb.cache
-
-
-def test_accelerate_replaces_every_layer_class():
+def test_accelerate_replaces_every_layer_class_and_patches_nothing():
     from transformers import GroundingDinoConfig, GroundingDinoForObjectDetection
-    from transformers.models.grounding_dino.modeling_grounding_dino import (GroundingDinoDecoderLayer, GroundingDinoDeformableLayer,
-                                                                           GroundingDinoFusionLayer)
+    from transformers.models.grounding_dino import modeling_grounding_dino as mgd
 
     cfg = GroundingDinoConfig()
     cfg.encoder_layers = cfg.decoder_layers = 2
     m = GroundingDinoForObjectDetection(cfg)
     info = ga.accelerate(m)
     assert info["deformable_layers"] == 2 and info["fusion_layers"] == 2 and info["decoder_layers"] == 2 and info["linear"] > 20
-    left = [type(x).__name__ for x in m.modules() if isinstance(x, (GroundingDinoDecoderLayer, GroundingDinoDeformableLayer, GroundingDinoFusionLayer))]
+    replaced = (mgd.GroundingDinoDecoderLayer, mgd.GroundingDinoDeformableLayer, mgd.GroundingDinoFusionLayer,
+                mgd.MultiScaleDeformableAttention, mgd.GroundingDinoMultiscaleDeformableAttention)
+    left = [type(x).__name__ for x in m.modules() if isinstance(x, replaced)]
     assert not left, left
-    assert isinstance(m.model.text_backbone, ga.CachedTextBackbone)
+    assert mgd.torch is torch                      # no process-wide patch of the modelling module

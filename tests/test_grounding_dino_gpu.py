@@ -61,31 +61,6 @@ def test_predict_surface_and_outputs(pair):
     assert back.num_detections == det.num_detections
 
 
-@pytest.mark.parametrize("f16", [False, True])
-def test_msda_kernel_vs_torch_grid_sample(f16):
-    """vlfm_msda_forward against transformers' pure-PyTorch MultiScaleDeformableAttention (fp32 grid_sample).
-    Tolerance 2e-5 for fp32 values (same taps, different summation order), 2e-3 for fp16 values."""
-    from transformers.models.grounding_dino.modeling_grounding_dino import MultiScaleDeformableAttention
-    from vlfm_b200.vlm.gdino_accel import TcMSDA
-
-    torch.manual_seed(0)
-    shapes = [(60, 80), (30, 40), (15, 20), (8, 10)]
-    b, heads, hd, q, pts = 2, 8, 32, 777, 4
-    s = sum(h * w for h, w in shapes)
-    value = torch.randn(b, s, heads, hd, device="cuda")
-    loc = torch.rand(b, q, heads, len(shapes), pts, 2, device="cuda") * 1.3 - 0.15      # some samples fall outside: zero padding
-    loc[0, 0, 0, 0, 0] = torch.tensor([0.5 / 80, 0.5 / 60])                             # exact pixel centre
-    attw = torch.softmax(torch.randn(b, q, heads, len(shapes) * pts, device="cuda"), -1).view(b, q, heads, len(shapes), pts)
-    sp = torch.tensor(shapes, device="cuda")
-    start = torch.cat([sp.new_zeros(1), (sp[:, 0] * sp[:, 1]).cumsum(0)[:-1]])
-    ref = MultiScaleDeformableAttention()(value, sp, shapes, start, loc, attw, 64)
-    got = TcMSDA()(value.half() if f16 else value, sp, shapes, start, loc, attw, 64)
-    torch.cuda.synchronize()
-    err = float((got - ref).abs().max())
-    print("msda max abs err", err)
-    assert got.shape == ref.shape and err <= (2e-3 if f16 else 2e-5)
-
-
 def test_tc_linear_and_cast_vs_torch():
     from vlfm_b200.vlm.dense import cast_f16
     from vlfm_b200.vlm.gdino_accel import TcLinear
@@ -253,7 +228,7 @@ def test_decoder_layer_vs_hf_module():
 
 def test_batch1_cuda_graph_replay_matches_eager(pair):
     """The per-step policy call (batch 1) replays a CUDA graph of the whole detector from the second call on; its outputs must
-    be those of the eager module graph.  With random weights the 900-of-6380 query selection is a top-k over near-tied scores,
+    be those of the eager forward.  With random weights the 900-of-6380 query selection is a top-k over near-tied scores,
     so even two EAGER runs differ (fp32 atomics order in the split-K GEMMs flips selections): the graph-vs-eager difference is
     held to the same level as eager-vs-eager, measured here on the spot (sorted confidences, boxes as sets)."""
     import time
@@ -317,8 +292,7 @@ def test_detection_decisions_match_the_fp32_twin(pair_calibrated):
     EPS16 = 2.0 ** -11
     cap = {}
     h1 = orc.model.model.decoder.register_forward_hook(lambda m_, a_, kw, o_: cap.__setitem__("ref", kw["reference_points"][0].detach().float().cpu()), with_kwargs=True)
-    h2 = g.model.model.decoder.register_forward_hook(lambda m_, a_, kw, o_: cap.__setitem__("got", kw["reference_points"][0].detach().float().cpu()), with_kwargs=True)
-    graph_ok, g._graph_ok = g._graph_ok, False                                  # eager: the hook must see the decoder call
+    graph_ok, g._graph_ok = g._graph_ok, False                                  # eager: every call sets g.fwd.last_reference_points
     stats = {"ours": [0, 0, 0, [], []], "twin": [0, 0, 0, [], []]}              # paired, unpaired, flipped, |dscore|, box L1
     try:
         for seed, caption in ((21, "chair . person . dog ."), (22, "couch . potted plant . tv .")):
@@ -327,7 +301,7 @@ def test_detection_decisions_match_the_fp32_twin(pair_calibrated):
             ref_l, ref_b = (t.cpu().float() for t in orc.raw_outputs(img, ids))
             ref_p = cap["ref"]
             got_l, got_b = (t.cpu().float() for t in g.raw_outputs(img, ids))
-            got_p = g.fwd.last_reference_points[0].detach().float().cpu() if g.fwd is not None else cap["got"]   # own forward keeps its own
+            got_p = g.fwd.last_reference_points[0].detach().float().cpu()
             per_l, per_b = (t.cpu().float() for t in orc.raw_outputs(img, ids, input_noise=EPS16, noise_seed=seed))
             per_p = cap["ref"]
             box_thr = float(ref_l.max(dim=1)[0].quantile(0.5))
@@ -353,7 +327,7 @@ def test_detection_decisions_match_the_fp32_twin(pair_calibrated):
                     st[3].append(abs(float(ref_l[i].max()) - float(dl[k].max())))
                     st[4].append(float((ref_b[i] - db[k]).abs().sum()))
     finally:
-        h1.remove(); h2.remove(); g._graph_ok = graph_ok
+        h1.remove(); g._graph_ok = graph_ok
     rep = {}
     for name, st in stats.items():
         rep[name] = {"paired": st[0], "unpaired": st[1], "flipped": st[2] / max(st[0], 1), "dscore": float(np.mean(st[3])), "dbox": float(np.mean(st[4]))}
@@ -437,23 +411,3 @@ def test_head_kernels_vs_torch():
     assert lg.shape == (B, 900, 256) and float(lg[..., T:].abs().max()) == 0.0
     assert float((lg[..., :T] - (hs @ tx.transpose(1, 2)).sigmoid()).abs().max()) <= 1e-5
 
-
-def test_own_forward_matches_the_module_graph(pair):
-    """GroundingDINO.raw_outputs through vlm/gdino_forward.py (own model-level forward) vs the same weights through HF's
-    GroundingDinoModel.forward on the same kernels (VLFM_GDINO_OWN_FORWARD=0 path): same proposals, same outputs up to the fp16
-    operand rounding of the few ops that differ (neck GEMM instead of cuDNN conv)."""
-    orc, g = pair
-    assert g.fwd is not None
-    img = make_rgb(np.random.default_rng(9), 480, 640)
-    ids = g.tokenizer.encode("chair . person . dog .")
-    a_l, a_b = (t.clone() for t in g.raw_outputs(img, ids))
-    fwd, g.fwd = g.fwd, None
-    g._static.clear()
-    try:
-        b_l, b_b = (t.clone() for t in g.raw_outputs(img, ids))
-    finally:
-        g.fwd = fwd
-        g._static.clear()
-    d = (a_b[:, None, :] - b_b[None, :, :]).abs().sum(-1).min(dim=1)[0]
-    print("own forward vs module graph: box set distance mean", float(d.mean()), "logit mean abs diff", float((a_l - b_l).abs().mean()))
-    assert float(d.mean()) <= 2e-2 and float((a_l - b_l).abs().mean()) <= 1e-2

@@ -57,7 +57,6 @@ _SIGNATURES = {
     "vlfm_value_disc_median_batch": (C.c_int, [C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "vlfm_obstacle_update": (C.c_int, [C.POINTER(ObstacleParams), C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "vlfm_value_cone_template": (C.c_int, [C.c_double, C.c_double, C.c_int, C.c_double, _P, _P, C.c_size_t, _P]),
-    "vlfm_msda_forward": (C.c_int, [_P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "vlfm_biattn_f16": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _P]),
     "vlfm_cast_f32_f16": (C.c_int, [_P, _P, C.c_long, _P]),
     "vlfm_cast_addpos_f16": (C.c_int, [_P, _P, _P, _P, C.c_long, _P]),

@@ -14,65 +14,6 @@ struct MsdaArgs {
   int H[MSDA_MAX_LEVELS], W[MSDA_MAX_LEVELS], start[MSDA_MAX_LEVELS];
 };
 
-template <typename T> __device__ __forceinline__ float ld_val(const T* p);
-template <> __device__ __forceinline__ float ld_val<float>(const float* p) { return __ldg(p); }
-template <> __device__ __forceinline__ float ld_val<__half>(const __half* p) { return __half2float(__ldg(p)); }
-
-// one warp per (b, q, head); lane = channel (hd <= 32 per pass).  Every tap is one coalesced hd*sizeof(T) read.
-template <typename T>
-__global__ void __launch_bounds__(256)
-msda_kernel(const T* __restrict__ value, const float* __restrict__ loc, const float* __restrict__ attw, float* __restrict__ out, MsdaArgs a) {
-  const int lane = threadIdx.x & 31;
-  const long warp = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const long total = (long)a.B * a.Q * a.heads;
-  if (warp >= total) return;
-  const int h = (int)(warp % a.heads);
-  const long bq = warp / a.heads;
-  const int b = (int)(bq / a.Q);
-  const int LP = a.levels * a.points;
-  const float* lp = loc + warp * LP * 2;
-  const float* wp = attw + warp * LP;
-  const T* vb = value + (size_t)b * a.S * a.heads * a.hd + (size_t)h * a.hd;
-  const size_t vstride = (size_t)a.heads * a.hd;
-  for (int c0 = 0; c0 < a.hd; c0 += 32) {
-    const int c = c0 + lane;
-    const bool cv = c < a.hd;
-    float acc = 0.f;
-    for (int j0 = 0; j0 < LP; j0 += 16) {                      // 16 (level, point) pairs per coalesced 128-byte load
-      const int nj = min(16, LP - j0);
-      const float mine = lane < 2 * nj ? __ldg(lp + 2 * j0 + lane) : 0.f;
-      const float wmine = lane < nj ? __ldg(wp + j0 + lane) : 0.f;
-      for (int jj = 0; jj < nj; ++jj) {
-        const float x = __shfl_sync(0xffffffffu, mine, 2 * jj), y = __shfl_sync(0xffffffffu, mine, 2 * jj + 1);
-        const float w = __shfl_sync(0xffffffffu, wmine, jj);
-        const int l = (j0 + jj) / a.points;
-        int Wl = a.W[0], Hl = a.H[0], lstart = a.start[0];
-#pragma unroll
-        for (int k = 1; k < MSDA_MAX_LEVELS; ++k)
-          if (l >= k) { Wl = a.W[k]; Hl = a.H[k]; lstart = a.start[k]; }
-        // HF: grid = 2*loc - 1 ; grid_sample: ((grid + 1) / 2) * size - 0.5   (no FMA contraction)
-        const float gx = __fsub_rn(__fmul_rn(2.f, x), 1.f), gy = __fsub_rn(__fmul_rn(2.f, y), 1.f);
-        const float ix = __fsub_rn(__fmul_rn(__fdiv_rn(__fadd_rn(gx, 1.f), 2.f), (float)Wl), 0.5f);
-        const float iy = __fsub_rn(__fmul_rn(__fdiv_rn(__fadd_rn(gy, 1.f), 2.f), (float)Hl), 0.5f);
-        const float fx0 = floorf(ix), fy0 = floorf(iy);
-        const int x0 = (int)fx0, y0 = (int)fy0;
-        const float tx = ix - fx0, ty = iy - fy0;
-        const float w00 = (1.f - tx) * (1.f - ty), w01 = tx * (1.f - ty), w10 = (1.f - tx) * ty, w11 = tx * ty;
-        const bool xin0 = x0 >= 0 && x0 < Wl, xin1 = x0 + 1 >= 0 && x0 + 1 < Wl, yin0 = y0 >= 0 && y0 < Hl, yin1 = y0 + 1 >= 0 && y0 + 1 < Hl;
-        if (!cv || !((xin0 || xin1) && (yin0 || yin1))) continue;
-        const T* base = vb + (size_t)lstart * vstride + c;
-        float s = 0.f;
-        if (yin0 && xin0) s += w00 * ld_val<T>(base + (size_t)(y0 * Wl + x0) * vstride);
-        if (yin0 && xin1) s += w01 * ld_val<T>(base + (size_t)(y0 * Wl + x0 + 1) * vstride);
-        if (yin1 && xin0) s += w10 * ld_val<T>(base + (size_t)((y0 + 1) * Wl + x0) * vstride);
-        if (yin1 && xin1) s += w11 * ld_val<T>(base + (size_t)((y0 + 1) * Wl + x0 + 1) * vstride);
-        acc += w * s;
-      }
-    }
-    if (cv) out[(size_t)warp * a.hd + c] = acc;
-  }
-}
-
 // Fused deformable attention for head_dim 32 / fp16 values.  One warp per (b, q, head).  Lanes 0-15 own one (level, point)
 // pair each for the softmax and the location arithmetic; the gather runs with lane = (tap = lane >> 3, channel quad =
 // lane & 7): all four bilinear taps of a point are ONE 8-byte load per lane, the taps are summed by two shuffles at the end.
@@ -358,28 +299,6 @@ __global__ void biattn_merge_kernel(const float* __restrict__ part, __half* __re
 }  // namespace vlfm
 
 using namespace vlfm;
-
-extern "C" int vlfm_msda_forward(const void* d_value, int value_is_f16, const float* d_loc, const float* d_attw, float* d_out, int B, int S,
-                                 int Q, int heads, int hd, int levels, int points, const int32_t* h_shapes_hw, void* stream) {
-  if (!d_value || !d_loc || !d_attw || !d_out || !h_shapes_hw || B < 1 || S < 1 || Q < 1 || heads < 1 || hd < 1 || points < 1 ||
-      levels < 1 || levels > MSDA_MAX_LEVELS) {
-    set_error("vlfm_msda_forward: bad argument"); return VLFM_E_INVALID;
-  }
-  MsdaArgs a{};
-  a.B = B; a.S = S; a.Q = Q; a.heads = heads; a.hd = hd; a.levels = levels; a.points = points;
-  int acc = 0;
-  for (int l = 0; l < levels; ++l) { a.H[l] = h_shapes_hw[2 * l]; a.W[l] = h_shapes_hw[2 * l + 1]; a.start[l] = acc; acc += a.H[l] * a.W[l]; }
-  if (acc != S) { set_error("vlfm_msda_forward: spatial shapes sum to %d, value has %d positions", acc, S); return VLFM_E_INVALID; }
-  const long warps = (long)B * Q * heads;
-  const long blocks = (warps + 7) / 8;
-  if (blocks > 0x7fffffffL) { set_error("vlfm_msda_forward: too many queries"); return VLFM_E_INVALID; }
-  cudaStream_t st = (cudaStream_t)stream;
-  if (value_is_f16) msda_kernel<__half><<<(unsigned)blocks, 256, 0, st>>>((const __half*)d_value, d_loc, d_attw, d_out, a);
-  else msda_kernel<float><<<(unsigned)blocks, 256, 0, st>>>((const float*)d_value, d_loc, d_attw, d_out, a);
-  VLFM_CHECK_LAUNCH("vlfm_msda_forward");
-  count_launch();
-  return VLFM_OK;
-}
 
 extern "C" int vlfm_cast_f32_f16(const float* d_in, void* d_out16, long n, void* stream) {
   if (!d_in || !d_out16 || n < 0) { set_error("vlfm_cast_f32_f16: bad argument"); return VLFM_E_INVALID; }

@@ -1,12 +1,13 @@
 """Hand-written kernels under the GroundingDINO feature enhancer / decoder (SURVEY.md 8f rank 1).
 
-The module graph (fusion layers, deformable encoder, decoder, heads) is still HF's
-``GroundingDinoForObjectDetection``; this file swaps its two hot primitives for the library's own kernels:
+``accelerate`` swaps the layers of HF's ``GroundingDinoForObjectDetection`` in place for classes that run on the library's
+own kernels; ``gdino_forward.GdinoForward`` then sequences them:
 
-* every ``nn.Linear``  -> ``TcLinear``: fp16 operands on the wgmma GEMM (csrc/gemm_wgmma.cu), fp32 accumulate,
-  bias fused, fp32 out (the reference runs these in fp32 SIMT GEMMs: groundingdino ... nn.Linear);
-* ``MultiScaleDeformableAttention`` (groundingdino's ms_deform_attn_cuda.cu / HF's grid_sample fallback)
-  -> ``vlfm_msda_forward`` (csrc/gdino_ops.cu).
+* ``GroundingDinoDeformableLayer`` -> ``TcDeformableLayer``, ``GroundingDinoFusionLayer`` -> ``TcFusionLayer``,
+  ``GroundingDinoDecoderLayer`` -> ``TcDecoderLayer``: GEMMs, fused multi-scale deformable sampling (``vlfm_msda_fused``,
+  replacing groundingdino's ms_deform_attn_cuda.cu) and bi-attention (``vlfm_biattn_f16``), csrc/gdino_ops.cu;
+* every other ``nn.Linear`` whose shape the GEMM takes -> ``TcLinear``: fp16 operands on the wgmma GEMM (csrc/gemm_wgmma.cu),
+  fp32 accumulate, bias fused, fp32 out (the reference runs these in fp32 SIMT GEMMs: groundingdino ... nn.Linear).
 """
 from __future__ import annotations
 
@@ -43,26 +44,6 @@ class TcLinear(torch.nn.Module):
         if x2.shape[0]:                 # the GEMM refuses M = 0
             gemm_f16(x2, self.w16, self.b32, _lib.EPI_BIAS_F32, out)
         return out.view(*shp[:-1], self.out_features)
-
-
-class TcMSDA(torch.nn.Module):
-    """Same call signature as transformers' ``MultiScaleDeformableAttention.forward``."""
-
-    def forward(self, value, value_spatial_shapes, value_spatial_shapes_list, level_start_index, sampling_locations, attention_weights,
-                im2col_step=None):
-        b, s, heads, hd = value.shape
-        _, q, _, levels, points, _ = sampling_locations.shape
-        value = value.contiguous()
-        assert value.dtype in (torch.float32, torch.float16)
-        loc = sampling_locations.float().contiguous()
-        attw = attention_weights.float().contiguous()
-        out = torch.empty((b, q, heads * hd), dtype=torch.float32, device=value.device)
-        flat = [int(v) for hw in value_spatial_shapes_list for v in hw]
-        shapes = (ctypes.c_int32 * len(flat))(*flat)
-        rc = _lib.load().vlfm_msda_forward(value.data_ptr(), int(value.dtype == torch.float16), loc.data_ptr(), attw.data_ptr(), out.data_ptr(),
-                                          b, s, q, heads, hd, levels, points, ctypes.cast(shapes, ctypes.c_void_p), _lib.stream_ptr())
-        _lib.check(rc, "vlfm_msda_forward")
-        return out
 
 
 def _w16(lin: torch.nn.Linear):
@@ -223,14 +204,14 @@ class TcFusionLayer(torch.nn.Module):
 class TcDecoderLayer(torch.nn.Module):
     """``GroundingDinoDecoderLayer.forward`` (self-attention over the 900 queries, text cross-attention, deformable image
     cross-attention, FFN; post-LN) on the library's kernels.  Attention masks are not supported (``self_attn_mask`` is None
-    at inference and captions are never padded on this path); a non-None ``self_attn_mask`` falls back to the original."""
+    at inference and captions are never padded on this path); neither are attention outputs."""
 
     def __init__(self, m):
         super().__init__()
         sa, ta = m.self_attn, m.encoder_attn_text
         assert sa.attention_head_size == 32 and ta.attention_head_size == 32
         self.heads = sa.num_attention_heads
-        self.deform = m.encoder_attn if isinstance(m.encoder_attn, TcDeformAttn) else TcDeformAttn(m.encoder_attn)
+        self.deform = TcDeformAttn(m.encoder_attn)
         wq, bq = _w16(sa.query); wk, bk = _w16(sa.key); wv, bv = _w16(sa.value); wo, bo = _w16(sa.out_proj)
         tq, tbq = _w16(ta.query); tk, tbk = _w16(ta.key); tv, tbv = _w16(ta.value); to, tbo = _w16(ta.out_proj)
         w1, b1 = _w16(m.fc1); w2, b2 = _w16(m.fc2)
@@ -243,15 +224,11 @@ class TcDecoderLayer(torch.nn.Module):
             self.eps.append(ln.eps)
         for n, t in bufs.items():
             self.register_buffer(n, t, persistent=False)
-        self.orig = [m]
 
     def forward(self, hidden_states, position_embeddings=None, reference_points=None, spatial_shapes=None, spatial_shapes_list=None,
                 level_start_index=None, vision_encoder_hidden_states=None, vision_encoder_attention_mask=None,
                 text_encoder_hidden_states=None, text_encoder_attention_mask=None, self_attn_mask=None, output_attentions=False):
-        if self_attn_mask is not None or output_attentions:
-            return self.orig[0](hidden_states, position_embeddings, reference_points, spatial_shapes, spatial_shapes_list, level_start_index,
-                                vision_encoder_hidden_states, vision_encoder_attention_mask, text_encoder_hidden_states,
-                                text_encoder_attention_mask, self_attn_mask, output_attentions)
+        assert self_attn_mask is None and not output_attentions
         b, nq, d = hidden_states.shape
         t = text_encoder_hidden_states.shape[1]
         scale = 32 ** -0.5
@@ -288,73 +265,12 @@ class TcDecoderLayer(torch.nn.Module):
         return (y.view(b, nq, d),)
 
 
-class CachedTextBackbone(torch.nn.Module):
-    """The BERT text tower depends only on the caption: its output is computed once per (caption ids, batch) and reused
-    (the reference re-runs it for every frame: groundingdino ... predict -> model(image, captions=[caption]))."""
-
-    def __init__(self, inner: torch.nn.Module, max_entries: int = 8):
-        super().__init__()
-        self.inner = inner
-        self.key = None                  # set by GroundingDINO.raw_outputs_device before every forward
-        self.cache: dict = {}
-        self.max_entries = max_entries
-
-    def forward(self, *args, **kwargs):
-        if self.key is None:
-            return self.inner(*args, **kwargs)
-        if self.key not in self.cache:
-            if len(self.cache) >= self.max_entries:
-                self.cache.pop(next(iter(self.cache)))
-            self.cache[self.key] = self.inner(*args, **kwargs)
-        return self.cache[self.key]
-
-
-class _TorchProxy:
-    """Stands in for the ``torch`` module inside transformers' GroundingDINO modelling file so that the handful of
-    host-list -> device tensor constructions in its forward (spatial shapes, special-token ids) are served from a cache
-    instead of issuing a synchronous H2D copy every call -- which is also what makes the forward CUDA-graph capturable."""
-
-    def __init__(self, real):
-        object.__setattr__(self, "_real", real)
-        object.__setattr__(self, "_cache", {})
-
-    def __getattr__(self, name):
-        return getattr(self._real, name)
-
-    def _cached(self, fn, data, args, kwargs):
-        dev = kwargs.get("device", None)
-        if isinstance(data, (list, tuple, int, float)) and dev is not None and self._real.device(dev).type == "cuda":
-            key = (fn.__name__, repr(data), str(kwargs.get("dtype", None)), str(dev))
-            hit = self._cache.get(key)
-            if hit is None:
-                hit = fn(data, *args, **kwargs)
-                self._cache[key] = hit
-            return hit
-        return fn(data, *args, **kwargs)
-
-    def as_tensor(self, data, *args, **kwargs):
-        return self._cached(self._real.as_tensor, data, args, kwargs)
-
-    def tensor(self, data, *args, **kwargs):
-        return self._cached(self._real.tensor, data, args, kwargs)
-
-
-def install_torch_proxy() -> None:
-    import transformers.models.grounding_dino.modeling_grounding_dino as mgd
-
-    if not isinstance(mgd.torch, _TorchProxy):
-        mgd.torch = _TorchProxy(mgd.torch)
-
-
 def accelerate(model: torch.nn.Module, min_out: int = 16) -> dict:
-    """Swap the primitives in place (model already on the GPU).  Returns counts for the log / tests."""
-    from transformers.models.grounding_dino.modeling_grounding_dino import (GroundingDinoDeformableLayer,
-                                                                           GroundingDinoMultiscaleDeformableAttention,
-                                                                           MultiScaleDeformableAttention)
+    """Swap the layers and linears in place (model already on the GPU).  Returns counts for the log / tests."""
+    from transformers.models.grounding_dino.modeling_grounding_dino import (GroundingDinoDecoderLayer, GroundingDinoDeformableLayer,
+                                                                           GroundingDinoFusionLayer)
 
-    from transformers.models.grounding_dino.modeling_grounding_dino import GroundingDinoDecoderLayer, GroundingDinoFusionLayer
-
-    n_lin = n_msda = n_skip = n_layer = n_attn = n_fuse = n_dec = 0
+    n_lin = n_skip = n_layer = n_fuse = n_dec = 0
     assert getattr(model.config, "activation_function", "relu") == "relu"
     for parent in list(model.modules()):
         for name, child in list(parent.named_children()):
@@ -366,18 +282,9 @@ def accelerate(model: torch.nn.Module, min_out: int = 16) -> dict:
                 setattr(parent, name, TcDecoderLayer(child)); n_dec += 1
     for parent in list(model.modules()):
         for name, child in list(parent.named_children()):
-            if isinstance(child, GroundingDinoMultiscaleDeformableAttention):
-                setattr(parent, name, TcDeformAttn(child)); n_attn += 1
-    for parent in list(model.modules()):
-        for name, child in list(parent.named_children()):
             if isinstance(child, torch.nn.Linear):
                 if child.in_features % 8 == 0 and child.in_features >= 16 and child.out_features >= min_out and child.out_features % 4 == 0:
                     setattr(parent, name, TcLinear(child)); n_lin += 1
                 else:
                     n_skip += 1
-            elif isinstance(child, MultiScaleDeformableAttention):
-                setattr(parent, name, TcMSDA()); n_msda += 1
-    if hasattr(model, "model") and hasattr(model.model, "text_backbone"):
-        model.model.text_backbone = CachedTextBackbone(model.model.text_backbone)
-        install_torch_proxy()
-    return {"linear": n_lin, "linear_kept": n_skip, "msda": n_msda, "deformable_layers": n_layer, "deformable_attn": n_attn, "fusion_layers": n_fuse, "decoder_layers": n_dec}
+    return {"linear": n_lin, "linear_kept": n_skip, "deformable_layers": n_layer, "fusion_layers": n_fuse, "decoder_layers": n_dec}

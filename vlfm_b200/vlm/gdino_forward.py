@@ -145,10 +145,7 @@ class GdinoForward:
         self_masks, position_ids = generate_masks_with_special_tokens_and_transfer_map(ids)
         tt = torch.zeros_like(ids)
         token_mask = torch.ones_like(ids).bool()
-        tb = core.text_backbone
-        if hasattr(tb, "key"):
-            tb.key = None                                  # CachedTextBackbone (gdino_accel): this class keeps its own per-caption cache
-        out = tb(ids, self_masks[:, None, :, :], tt, position_ids, return_dict=True)
+        out = core.text_backbone(ids, self_masks[:, None, :, :], tt, position_ids, return_dict=True)
         feats = out.last_hidden_state.float()
         T = feats.shape[1]
         proj = self.ops.linear(feats.reshape(B * T, -1), self.text_proj_w, self.text_proj_b).view(B, T, self.d)

@@ -2,39 +2,29 @@
 
 The Swin-T backbone -- the dense contraction north_star names -- runs on the hand-written sm_90a kernels
 (``SwinBackboneEngine``); every nn.Linear, the deformable encoder layers, the image<->text fusion layers and the decoder layers
-run on the library too (``gdino_accel``: wgmma GEMM, fused multi-scale deformable sampling, bi-attention).  The module graph
-that sequences them is HF's ``GroundingDinoForObjectDetection`` (architecture-equivalent to groundingdino@eeba084); what is
-still PyTorch glue is listed in DESIGN.md section 7.  Post-processing restates groundingdino.util.inference.predict.
+run on the library too (``gdino_accel``: wgmma GEMM, fused multi-scale deformable sampling, bi-attention).  ``GdinoForward``
+(``gdino_forward``) sequences them -- neck, encoder loop, proposal selection, decoder loop, heads -- over the weights of HF's
+``GroundingDinoForObjectDetection`` (architecture-equivalent to groundingdino@eeba084); what is still PyTorch glue is listed in
+DESIGN.md section 7.  Post-processing restates groundingdino.util.inference.predict.
 """
 from __future__ import annotations
 
 import os
-from typing import Any, Callable, Dict, List, Optional
+from typing import Any, Dict, List, Optional
 
 import numpy as np
 import torch
 
 from .detections import ObjectDetections
 from .gdino_accel import accelerate
+from .gdino_forward import GdinoForward
+from .gdino_ops import LibOps
 from .swin_engine import SwinBackboneEngine
 
 GROUNDING_DINO_CONFIG = "GroundingDINO/groundingdino/config/GroundingDINO_SwinT_OGC.py"
 GROUNDING_DINO_WEIGHTS = "data/groundingdino_swint_ogc.pth"
 CLASSES = "chair . person . dog ."  # grounding_dino.py:20
 BACKBONE_PREFIX = "model.backbone.conv_encoder.model."
-
-
-class _Features(torch.nn.Module):
-    """Stands in for the HF backbone module: returns the feature maps our engine produced."""
-
-    def __init__(self):
-        super().__init__()
-        self.maps: List[torch.Tensor] = []
-
-    def forward(self, pixel_values=None, **kw):
-        from transformers.modeling_outputs import BackboneOutput
-
-        return BackboneOutput(feature_maps=tuple(self.maps))
 
 
 class SimpleCaptionTokenizer:
@@ -102,19 +92,14 @@ class GroundingDINO:
                                            depths=cfg.backbone_config.depths, heads=cfg.backbone_config.num_heads,
                                            out_stages=tuple(cfg.backbone_config.out_indices), eps=cfg.backbone_config.layer_norm_eps,
                                            device=device)
-        self._features = _Features()
-        model.model.backbone.conv_encoder.model = self._features
+        # the engine above holds the Swin weights; HF's copy would only occupy the device twice (GdinoForward reads just the
+        # backbone's position embedding)
+        model.model.backbone.conv_encoder.model = torch.nn.Identity()
         self.model = model.to(device).eval()
-        # feature enhancer / decoder: nn.Linear -> wgmma GEMM, deformable-attention sampling -> vlfm_msda_forward
-        self.accel = accelerate(self.model) if os.environ.get("VLFM_GDINO_ACCEL", "1") != "0" else {}
-        # model-level glue (neck, proposal scoring, top-900 selection, heads) on the library's kernels; VLFM_GDINO_OWN_FORWARD=0 keeps
-        # HF's GroundingDinoModel.forward for A/B comparisons
-        self.fwd = None
-        if os.environ.get("VLFM_GDINO_OWN_FORWARD", "1") != "0":
-            from .gdino_forward import GdinoForward
-            from .gdino_ops import LibOps
-
-            self.fwd = GdinoForward(self.model, LibOps(), self.backbone)
+        # encoder / decoder layers and every nn.Linear on the library's kernels
+        self.accel = accelerate(self.model)
+        # model-level sequencing (neck, encoder loop, proposal selection, decoder loop, heads)
+        self.fwd = GdinoForward(self.model, LibOps(), self.backbone)
         self.caption = caption
         self.box_threshold = box_threshold
         self.text_threshold = text_threshold
@@ -145,36 +130,20 @@ class GroundingDINO:
 
     def _forward_static(self, st):
         """One forward on the static buffers of ``st`` (eager or under CUDA-graph capture)."""
-        if self.fwd is not None:
-            st["logits"], st["boxes"] = self.fwd.forward(st["img"], st["key_ids"])
-            st["keep"] = self.fwd.last       # a captured graph reads the cached shape / caption constants by address: keep them alive
-            return
-        self._features.maps = self.backbone.forward(st["img"])
-        out = self.model(pixel_values=st["dummy"], input_ids=st["ids"], token_type_ids=st["tt"], attention_mask=st["am"], pixel_mask=st["pm"])
-        st["logits"], st["boxes"] = out.logits.sigmoid(), out.pred_boxes
-        # a captured graph reads the cached text-tower output by ADDRESS: this entry owns a reference, so evicting the caption
-        # from the text cache (FIFO, 8 entries) can never free memory a live graph replays from
-        tb = self.model.model.text_backbone
-        if hasattr(tb, "cache"):
-            st["text_ref"] = tb.cache.get(tb.key)
+        st["logits"], st["boxes"] = self.fwd.forward(st["img"], st["key_ids"])
+        st["keep"] = self.fwd.last       # a captured graph reads the cached shape / caption constants by address: keep them alive
 
     @torch.inference_mode()
     def raw_outputs_device(self, images: torch.Tensor, input_ids: List[int]):
         """images [B,H,W,3] uint8 on the device -> (sigmoid logits [B,900,256], boxes [B,900,4] cxcywh).
 
         Small batches (the per-step policy call is batch 1) replay a CUDA graph of the whole detector per
-        (batch, image size, caption): the module graph is ~700 launches and launch-bound otherwise."""
+        (batch, image size, caption): the forward is launch-bound otherwise."""
         b, h, w = images.shape[:3]
         key = (int(b), int(h), int(w), tuple(int(i) for i in input_ids))
-        tb = self.model.model.text_backbone
-        if hasattr(tb, "key"):
-            tb.key = (key[3], key[0])
         st = self._static.get(key)
         if st is None:
-            ids = torch.tensor([list(key[3])], dtype=torch.long, device=self.device).expand(b, -1).contiguous()
-            st = {"img": torch.empty_like(images), "ids": ids, "tt": torch.zeros_like(ids), "am": torch.ones_like(ids),
-                  "dummy": torch.zeros(b, 3, h, w, device=self.device),   # only its shape is used (pixel mask); features come from our engine
-                  "pm": torch.ones(b, h, w, dtype=torch.long, device=self.device), "calls": 0, "graph": None, "key_ids": list(key[3])}
+            st = {"img": torch.empty_like(images), "calls": 0, "graph": None, "key_ids": list(key[3])}
             if len(self._static) >= 4:
                 self._static.pop(next(iter(self._static)))
             self._static[key] = st
@@ -188,7 +157,7 @@ class GroundingDINO:
                 with torch.cuda.graph(g):
                     self._forward_static(st)
                 st["graph"] = g
-            except Exception as e:  # a sync point inside the module graph: stay eager (loudly, once)
+            except Exception as e:  # a sync point inside the forward: stay eager (loudly, once)
                 self._graph_ok = False
                 self.graph_error = repr(e)
                 print(f"[vlfm_b200] GroundingDINO CUDA-graph capture disabled: {e}", flush=True)
