@@ -400,8 +400,9 @@ int vlfm_render_draw(int G, int batch, uint8_t* d_frames, const int32_t* h_lists
  * attentions run on vlfm_gemm_f16 / vlfm_gemm_f16_resid_ln / vlfm_layernorm / vlfm_attention_f16; these are the rest.
  *
  * vlfm_sam_preprocess: ResizeLongestSide(S): Pillow-exact bilinear resize [B,H,W,3] uint8 -> (OH, OW) (tables as for
- *   vlfm_preprocess_im2col, built by vlm/preprocess.py::bilinear_tables; d_mid [B,H,OW,3] uint8 scratch), then
- *   (x - mean) / std in fp32 (h_mean3 / h_std3: HOST float[3] on the 0..255 scale) and a zero pad to S x S -> d_out [B,S,S,3] fp16.
+ *   vlfm_preprocess_im2col, built by vlm/preprocess.py::bilinear_tables), horizontal pass first into d_mid [B,H,OW,3] uint8
+ *   scratch, or with v_first = 1 (Pillow's order for frames more than 100x taller than wide that shrink vertically, see
+ *   vlm/preprocess.py::pillow_vertical_first) vertical first into d_mid [B,OH,W,3]; then (x - mean) / std in fp32 (h_mean3 / h_std3: HOST float[3] on the 0..255 scale) and a zero pad to S x S -> d_out [B,S,S,3] fp16.
  * vlfm_sam_im2col3x3: fp16 NHWC [B,H,W,C] -> fp16 [B*Ho*Wo, ldk] rows of a 3x3 conv (pad 1, stride 1 or 2), column (ky*3+kx)*C + c,
  *   columns >= 9*C zero.  ldk % 8 == 0.
  * vlfm_sam_dwconv3x3: depthwise 3x3 conv (pad 1, stride 1 or 2), NHWC, weights d_w [9, C] (tap-major, BatchNorm folded) + d_b [C],
@@ -426,7 +427,7 @@ int vlfm_render_draw(int G, int batch, uint8_t* d_frames, const int32_t* h_lists
  *   to (H, W) -> > 0 -> d_out [M, H, W] uint8. */
 int vlfm_sam_preprocess(const uint8_t* d_img, uint8_t* d_mid, void* d_out, int B, int H, int W, int OH, int OW, int S,
                         const int32_t* d_hbounds, const int32_t* d_hkk, int hksize, const int32_t* d_vbounds, const int32_t* d_vkk,
-                        int vksize, const float* h_mean3, const float* h_std3, void* stream);
+                        int vksize, int v_first, const float* h_mean3, const float* h_std3, void* stream);
 int vlfm_sam_im2col3x3(const void* d_x16, void* d_col16, int B, int H, int W, int C, int stride, int ldk, void* stream);
 int vlfm_sam_dwconv3x3(const void* d_in, int in_f32, const float* d_w, const float* d_b, void* d_out, int out_f32, int B, int H, int W,
                        int C, int stride, int gelu, void* stream);

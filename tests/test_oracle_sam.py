@@ -1,5 +1,5 @@
-"""CPU checks of MobileSAM's host-side pieces: the Pillow-exact bilinear tables, BatchNorm folding, and the oracle's TinyViT
-window attention."""
+"""CPU checks of MobileSAM's host-side pieces: the Pillow-exact bilinear tables and pass order, BatchNorm folding, and the
+oracle's TinyViT window attention."""
 import numpy as np
 import pytest
 import torch
@@ -7,7 +7,7 @@ import torch.nn.functional as F
 from torchvision.transforms.functional import resize, to_pil_image
 
 from oracle.sam_oracle import SamOracle, preprocess, preshape
-from vlfm_b200.vlm.preprocess import bilinear_tables, resize_numpy
+from vlfm_b200.vlm.preprocess import bilinear_tables, pillow_vertical_first, resize_numpy
 from vlfm_b200.vlm.sam_config import TINY, random_state_dict
 from vlfm_b200.vlm.sam_weights import fold_conv_bn, offset_index
 
@@ -20,6 +20,47 @@ def test_bilinear_tables_match_pillow(hw):
     newh, neww = preshape(hw[0], hw[1], 1024)
     ref = np.array(resize(to_pil_image(img), [newh, neww]))
     assert np.array_equal(resize_numpy(img, newh, neww, tables=bilinear_tables), ref)
+
+
+# Sides 1..2048 around the pass-order switch (height > 100 x width and shrinking vertically): the frames that are at most
+# 11 px wide and 1000..2048 px tall, both orientations of each, and camera-like sizes.  The first list is where a
+# horizontal-first resize differs from Pillow's bytes.
+VERTICAL_FIRST_DIFFERS = [(1200, 7), (1200, 8), (1536, 3), (1536, 7), (1536, 8), (2000, 3), (2000, 7), (2000, 8), (2048, 3), (2048, 7),
+                          (2048, 8)]
+SWEEP = sorted({(h, w) for h in (1, 2, 3, 99, 100, 101, 150, 700, 800, 801, 1000, 1024, 1025, 1100, 1101, 1200, 1536, 2000, 2048)
+                for w in (1, 2, 3, 4, 7, 8, 9, 10, 11, 12, 21, 640)} | {(w, h) for h in (1000, 1025, 1536, 2048) for w in (1, 3, 8, 11)}
+               | set(VERTICAL_FIRST_DIFFERS))
+
+
+def test_resize_pass_order_matches_pillow_sweep():
+    """resize_numpy (the GPU passes' order and arithmetic) byte-equal to Pillow on every size of SWEEP, each with the order
+    Pillow picks; on the listed tall, narrow frames the other order is not, so the order is what makes them pass."""
+    rng = np.random.default_rng(0)
+    switched = 0
+    for h, w in SWEEP:
+        img = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+        newh, neww = preshape(h, w, 1024)
+        ref = np.array(resize(to_pil_image(img), [newh, neww]))
+        assert np.array_equal(resize_numpy(img, newh, neww, tables=bilinear_tables), ref), (h, w)
+        switched += pillow_vertical_first(h, w, newh)
+    assert switched >= 30
+    for h, w in VERTICAL_FIRST_DIFFERS:
+        assert pillow_vertical_first(h, w, 1024)
+        img = np.random.default_rng(h + w).integers(0, 256, (h, w, 3), dtype=np.uint8)
+        newh, neww = preshape(h, w, 1024)
+        hb, hk, _ = bilinear_tables(w, neww)
+        vb, vk, _ = bilinear_tables(h, newh)
+        mid = np.stack([(img[:, b0:b0 + n].astype(np.int64) * k[:n, None]).sum(1) for (b0, n), k in zip(hb, hk)], 1)
+        mid = np.clip((mid + (1 << 21)) >> 22, 0, 255)
+        hfirst = np.stack([(mid[b0:b0 + n] * k[:n, None, None]).sum(0) for (b0, n), k in zip(vb, vk)], 0)
+        hfirst = np.clip((hfirst + (1 << 21)) >> 22, 0, 255)
+        assert not np.array_equal(hfirst, np.array(resize(to_pil_image(img), [newh, neww]))), (h, w)
+
+
+def test_pass_order_boundary():
+    assert pillow_vertical_first(1025, 10, 1024) and not pillow_vertical_first(1000, 10, 1024)
+    assert not pillow_vertical_first(1000, 8, 1024)          # taller than 100 x 8 but enlarged: horizontal first
+    assert not pillow_vertical_first(2048, 1536, 1024) and not pillow_vertical_first(8, 2000, 8)
 
 
 def test_bilinear_tables_downscale_support():

@@ -108,7 +108,7 @@ _SIGNATURES = {
     "vlfm_render_value": (C.c_int, [C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P, C.c_size_t, _P]),
     "vlfm_render_obstacle": (C.c_int, [C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "vlfm_render_draw": (C.c_int, [C.c_int, C.c_int, _P, _P, C.c_size_t, _P, C.c_size_t, _P]),
-    "vlfm_sam_preprocess": (C.c_int, [_P, _P, _P] + [C.c_int] * 6 + [_P, _P, C.c_int, _P, _P, C.c_int,
+    "vlfm_sam_preprocess": (C.c_int, [_P, _P, _P] + [C.c_int] * 6 + [_P, _P, C.c_int, _P, _P, C.c_int, C.c_int,
                                       C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
     "vlfm_sam_im2col3x3": (C.c_int, [_P, _P] + [C.c_int] * 6 + [_P]),
     "vlfm_sam_dwconv3x3": (C.c_int, [_P, C.c_int, _P, _P, _P] + [C.c_int] * 7 + [_P]),

@@ -2,8 +2,8 @@
 // Reference call site: vlfm/vlm/sam.py:40-57 (SamPredictor.set_image + predict(box=..., multimask_output=False)).
 // GEMMs, LayerNorms and the short attentions run on the shared kernels (vlfm_gemm_f16*, vlfm_layernorm, vlfm_attention_f16);
 // the engine is vlm/sam_engine.py.
-//   - sam_resize_h / sam_resize_v_norm: Pillow-exact separable bilinear resize (ResizeLongestSide(1024)), the fp32 pixel
-//     normalisation (true division) and the zero pad to S x S, written as fp16 NHWC;
+//   - sam_resize_pass / sam_resize_norm: Pillow-exact separable bilinear resize (ResizeLongestSide(1024)) in Pillow's pass
+//     order, the fp32 pixel normalisation (true division) and the zero pad to S x S, written as fp16 NHWC;
 //   - sam_im2col3x3: fp16 NHWC -> rows of a 3x3 (stride 1 or 2, pad 1) conv GEMM, K zero-padded to ldk;
 //   - sam_dwconv3x3: depthwise 3x3 conv with folded BatchNorm and optional GELU (TinyViT MBConv / PatchMerging / local_conv);
 //   - sam_add_act: out = act(a + b) (MBConv "add shortcut, then GELU"; plain casts);
@@ -35,28 +35,39 @@ static unsigned grid1d(long long n, int threads) {
 }
 
 // ---------------------------------------------------------------------------------------------------------- preprocess
-__global__ void sam_resize_h_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ mid, int B, int H, int W, int OW,
-                                    const int32_t* __restrict__ bounds, const int32_t* __restrict__ kk, int ksize) {
-  const long long n = (long long)B * H * OW;
+// One pixel of a Pillow 8-bpc pass along y (vert) or x: `in` is [B, inH, inW, 3] uint8 and (y, x) the output coordinate; the
+// taps of output index o = (vert ? y : x) start at bounds[2*o] and number bounds[2*o+1].
+__device__ __forceinline__ void sam_resample_px(const uint8_t* __restrict__ in, int b, int inH, int inW, int y, int x, int vert,
+                                                const int32_t* __restrict__ bounds, const int32_t* __restrict__ kk, int ksize,
+                                                uint8_t px[3]) {
+  const int o = vert ? y : x;
+  const int s0 = bounds[2 * o], cnt = bounds[2 * o + 1];
+  const int32_t* k = kk + (size_t)o * ksize;
+  const size_t step = vert ? (size_t)inW * 3 : 3;
+  const uint8_t* src = in + (((size_t)b * inH + (vert ? s0 : y)) * inW + (vert ? x : s0)) * 3;
+  int a0 = 1 << (SAM_PREC_BITS - 1), a1 = a0, a2 = a0;
+  for (int t = 0; t < cnt; ++t) {
+    const uint8_t* p = src + t * step;
+    const int c = k[t];
+    a0 += p[0] * c; a1 += p[1] * c; a2 += p[2] * c;
+  }
+  px[0] = sam_clip8(a0 >> SAM_PREC_BITS); px[1] = sam_clip8(a1 >> SAM_PREC_BITS); px[2] = sam_clip8(a2 >> SAM_PREC_BITS);
+}
+
+// first pass: [B, H, W, 3] -> mid [B, mH, mW, 3] along one axis (the other keeps its input size)
+__global__ void sam_resize_pass_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ mid, int B, int H, int W, int mH, int mW,
+                                       int vert, const int32_t* __restrict__ bounds, const int32_t* __restrict__ kk, int ksize) {
+  const long long n = (long long)B * mH * mW;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const int xo = (int)(i % OW);
-    const long long by = i / OW;   // b * H + y
-    const int x0 = bounds[2 * xo], cnt = bounds[2 * xo + 1];
-    const uint8_t* src = in + (by * W + x0) * 3;
-    const int32_t* k = kk + (size_t)xo * ksize;
-    int s0 = 1 << (SAM_PREC_BITS - 1), s1 = s0, s2 = s0;
-    for (int t = 0; t < cnt; ++t) {
-      const int c = k[t];
-      s0 += src[3 * t] * c; s1 += src[3 * t + 1] * c; s2 += src[3 * t + 2] * c;
-    }
-    uint8_t* o = mid + i * 3;
-    o[0] = sam_clip8(s0 >> SAM_PREC_BITS); o[1] = sam_clip8(s1 >> SAM_PREC_BITS); o[2] = sam_clip8(s2 >> SAM_PREC_BITS);
+    const int x = (int)(i % mW), y = (int)((i / mW) % mH), b = (int)(i / ((long long)mH * mW));
+    sam_resample_px(in, b, H, W, y, x, vert, bounds, kk, ksize, mid + i * 3);
   }
 }
 
-__global__ void sam_resize_v_norm_kernel(const uint8_t* __restrict__ mid, __half* __restrict__ out, int B, int H, int OH, int OW,
-                                         int S, const int32_t* __restrict__ bounds, const int32_t* __restrict__ kk, int ksize,
-                                         float m0, float m1, float m2, float s0, float s1, float s2) {
+// second pass along the other axis: mid [B, mH, mW, 3] -> (OH, OW), (x - mean) / std, zero pad -> out [B, S, S, 3] fp16
+__global__ void sam_resize_norm_kernel(const uint8_t* __restrict__ mid, __half* __restrict__ out, int B, int mH, int mW, int OH, int OW,
+                                       int S, int vert, const int32_t* __restrict__ bounds, const int32_t* __restrict__ kk, int ksize,
+                                       float m0, float m1, float m2, float s0, float s1, float s2) {
   const long long n = (long long)B * S * S;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const int x = (int)(i % S), y = (int)((i / S) % S), b = (int)(i / ((long long)S * S));
@@ -65,18 +76,12 @@ __global__ void sam_resize_v_norm_kernel(const uint8_t* __restrict__ mid, __half
       o[0] = o[1] = o[2] = __float2half_rn(0.f);
       continue;
     }
-    const int y0 = bounds[2 * y], cnt = bounds[2 * y + 1];
-    const int32_t* k = kk + (size_t)y * ksize;
-    int a0 = 1 << (SAM_PREC_BITS - 1), a1 = a0, a2 = a0;
-    for (int t = 0; t < cnt; ++t) {
-      const uint8_t* p = mid + (((size_t)b * H + y0 + t) * OW + x) * 3;
-      const int c = k[t];
-      a0 += p[0] * c; a1 += p[1] * c; a2 += p[2] * c;
-    }
+    uint8_t px[3];
+    sam_resample_px(mid, b, mH, mW, y, x, vert, bounds, kk, ksize, px);
     // (x - mean) / std in fp32 with a true division (segment_anything's Sam.preprocess)
-    o[0] = __float2half_rn(__fdiv_rn(__fsub_rn((float)sam_clip8(a0 >> SAM_PREC_BITS), m0), s0));
-    o[1] = __float2half_rn(__fdiv_rn(__fsub_rn((float)sam_clip8(a1 >> SAM_PREC_BITS), m1), s1));
-    o[2] = __float2half_rn(__fdiv_rn(__fsub_rn((float)sam_clip8(a2 >> SAM_PREC_BITS), m2), s2));
+    o[0] = __float2half_rn(__fdiv_rn(__fsub_rn((float)px[0], m0), s0));
+    o[1] = __float2half_rn(__fdiv_rn(__fsub_rn((float)px[1], m1), s1));
+    o[2] = __float2half_rn(__fdiv_rn(__fsub_rn((float)px[2], m2), s2));
   }
 }
 
@@ -405,17 +410,23 @@ using namespace vlfm;
 
 extern "C" int vlfm_sam_preprocess(const uint8_t* d_img, uint8_t* d_mid, void* d_out, int B, int H, int W, int OH, int OW, int S,
                                    const int32_t* d_hbounds, const int32_t* d_hkk, int hksize, const int32_t* d_vbounds,
-                                   const int32_t* d_vkk, int vksize, const float* h_mean3, const float* h_std3, void* stream) {
+                                   const int32_t* d_vkk, int vksize, int v_first, const float* h_mean3, const float* h_std3,
+                                   void* stream) {
   if (!d_img || !d_mid || !d_out || !d_hbounds || !d_hkk || !d_vbounds || !d_vkk || !h_mean3 || !h_std3 || B < 1 || H < 1 || W < 1 ||
-      OH < 1 || OW < 1 || OH > S || OW > S || hksize < 1 || vksize < 1) {
+      OH < 1 || OW < 1 || OH > S || OW > S || hksize < 1 || vksize < 1 || (v_first != 0 && v_first != 1)) {
     set_error("vlfm_sam_preprocess: bad argument"); return VLFM_E_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
-  sam_resize_h_kernel<<<grid1d((long long)B * H * OW, 256), 256, 0, st>>>(d_img, d_mid, B, H, W, OW, d_hbounds, d_hkk, hksize);
-  SAM_LAUNCHED("sam_resize_h_kernel");
-  sam_resize_v_norm_kernel<<<grid1d((long long)B * S * S, 256), 256, 0, st>>>(d_mid, (__half*)d_out, B, H, OH, OW, S, d_vbounds, d_vkk,
-                                                                                vksize, h_mean3[0], h_mean3[1], h_mean3[2], h_std3[0],
-                                                                                h_std3[1], h_std3[2]);
-  SAM_LAUNCHED("sam_resize_v_norm_kernel");
+  // Pillow resizes horizontally first, except for frames more than 100x taller than wide that shrink vertically
+  const int mH = v_first ? OH : H, mW = v_first ? W : OW;
+  const int32_t *b1 = v_first ? d_vbounds : d_hbounds, *k1 = v_first ? d_vkk : d_hkk;
+  const int32_t *b2 = v_first ? d_hbounds : d_vbounds, *k2 = v_first ? d_hkk : d_vkk;
+  sam_resize_pass_kernel<<<grid1d((long long)B * mH * mW, 256), 256, 0, st>>>(d_img, d_mid, B, H, W, mH, mW, v_first, b1, k1,
+                                                                              v_first ? vksize : hksize);
+  SAM_LAUNCHED("sam_resize_pass_kernel");
+  sam_resize_norm_kernel<<<grid1d((long long)B * S * S, 256), 256, 0, st>>>(d_mid, (__half*)d_out, B, mH, mW, OH, OW, S, !v_first, b2, k2,
+                                                                            v_first ? hksize : vksize, h_mean3[0], h_mean3[1], h_mean3[2],
+                                                                            h_std3[0], h_std3[1], h_std3[2]);
+  SAM_LAUNCHED("sam_resize_norm_kernel");
   return VLFM_OK;
 }
 

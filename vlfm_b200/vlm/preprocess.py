@@ -84,20 +84,30 @@ def bilinear_tables(in_size: int, out_size: int) -> Tuple[np.ndarray, np.ndarray
     return bounds, kk, ksize
 
 
+def pillow_vertical_first(in_h: int, in_w: int, out_h: int) -> bool:
+    """Pillow's pass order: ``Image.resize`` (Pillow 12.2, Image.py) resizes a frame more than 100x taller than wide that
+    shrinks vertically as a vertical resize to (in_w, out_h) followed by a horizontal one; every other frame goes through one
+    ``ImagingResample`` call, horizontal pass first.  The passes round to uint8 in between, so the order changes bytes."""
+    return in_h > in_w * 100 and out_h < in_h
+
+
+def _resize_pass(src: np.ndarray, out_n: int, tables, axis: int) -> np.ndarray:
+    """One fixed-point pass of [h, w, 3] int64 along axis 1 (horizontal) or 0 (vertical), clipped to 0..255."""
+    b, k, _ = tables(src.shape[axis], out_n)
+    t = np.moveaxis(src, axis, 1)
+    out = np.zeros((t.shape[0], out_n, 3), np.int64)
+    for o in range(out_n):
+        s0, n = b[o]
+        acc = (t[:, s0 : s0 + n, :] * k[o, :n][None, :, None].astype(np.int64)).sum(1) + (1 << (PRECISION_BITS - 1))
+        out[:, o, :] = np.clip(acc >> PRECISION_BITS, 0, 255)
+    return np.moveaxis(out, 1, axis)
+
+
 def resize_numpy(img: np.ndarray, out_h: int, out_w: int, tables=bicubic_tables) -> np.ndarray:
-    """Reference emulation of the two GPU passes (used by CPU tests to pin the tables to PIL)."""
-    h, w, _ = img.shape
-    hb, hk, _ = tables(w, out_w)
-    vb, vk, _ = tables(h, out_h)
+    """Reference emulation of the two GPU passes in Pillow's order (used by CPU tests to pin the tables to PIL)."""
     src = img.astype(np.int64)
-    mid = np.zeros((h, out_w, 3), np.int64)
-    for xo in range(out_w):
-        x0, n = hb[xo]
-        acc = (src[:, x0 : x0 + n, :] * hk[xo, :n][None, :, None].astype(np.int64)).sum(1) + (1 << (PRECISION_BITS - 1))
-        mid[:, xo, :] = np.clip(acc >> PRECISION_BITS, 0, 255)
-    out = np.zeros((out_h, out_w, 3), np.int64)
-    for yo in range(out_h):
-        y0, n = vb[yo]
-        acc = (mid[y0 : y0 + n] * vk[yo, :n][:, None, None].astype(np.int64)).sum(0) + (1 << (PRECISION_BITS - 1))
-        out[yo] = np.clip(acc >> PRECISION_BITS, 0, 255)
+    if pillow_vertical_first(img.shape[0], img.shape[1], out_h):
+        out = _resize_pass(_resize_pass(src, out_h, tables, 0), out_w, tables, 1)
+    else:
+        out = _resize_pass(_resize_pass(src, out_w, tables, 1), out_h, tables, 0)
     return out.astype(np.uint8)

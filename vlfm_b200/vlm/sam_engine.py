@@ -21,7 +21,7 @@ import torch
 
 from .. import _lib
 from .dense import attention_f16, gemm_f16, gemm_f16_resid_ln, layernorm
-from .preprocess import bilinear_tables
+from .preprocess import bilinear_tables, pillow_vertical_first
 from .sam_config import SamDims
 
 F16, F32 = torch.float16, torch.float32
@@ -100,7 +100,7 @@ class MobileSamEngine:
             hb, hk, hks = bilinear_tables(W, neww)
             vb, vk, vks = bilinear_tables(H, newh)
             t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(self.dev)
-            self._pre[key] = (newh, neww, t(hb), t(hk), hks, t(vb), t(vk), vks)
+            self._pre[key] = (newh, neww, t(hb), t(hk), hks, t(vb), t(vk), vks, int(pillow_vertical_first(H, W, newh)))
         return self._pre[key]
 
     def _enc_buffers(self, B: int) -> Dict[str, torch.Tensor]:
@@ -121,12 +121,12 @@ class MobileSamEngine:
     def preprocess(self, images: torch.Tensor) -> torch.Tensor:
         """[B,H,W,3] uint8 (device) -> [B,S,S,3] fp16: ResizeLongestSide, normalise, zero pad"""
         B, H, W, _ = images.shape
-        newh, neww, hb, hk, hks, vb, vk, vks = self._tables(H, W)
+        newh, neww, hb, hk, hks, vb, vk, vks, v_first = self._tables(H, W)
         buf = self._enc_buffers(B)
-        mid = torch.empty(B * H * neww * 3, dtype=torch.uint8, device=self.dev)
+        mid = torch.empty(B * (newh * W if v_first else H * neww) * 3, dtype=torch.uint8, device=self.dev)
         rc = self.lib.vlfm_sam_preprocess(images.data_ptr(), mid.data_ptr(), buf["img"].data_ptr(), B, H, W, newh, neww, self.d.img_size,
-                                          hb.data_ptr(), hk.data_ptr(), hks, vb.data_ptr(), vk.data_ptr(), vks, self._mean, self._std,
-                                          _lib.stream_ptr())
+                                          hb.data_ptr(), hk.data_ptr(), hks, vb.data_ptr(), vk.data_ptr(), vks, v_first, self._mean,
+                                          self._std, _lib.stream_ptr())
         _lib.check(rc, "vlfm_sam_preprocess")
         return buf["img"]
 
