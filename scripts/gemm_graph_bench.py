@@ -1,22 +1,34 @@
 """Per-shape GEMM timing at full clocks: 200 back-to-back launches captured in a CUDA graph
-(no CPU launch bound), optional sweep of the tile plan via VLFM_GEMM_FORCE=bn:splits."""
-import os, sys, itertools
+(no CPU launch bound), optional sweep of the tile plan via VLFM_GEMM_FORCE=bn:splits.
+
+The four ViT-g layer GEMMs at batch 1 run as the forward runs them: qkv and fc1 through vlfm_gemm_f16, proj and fc2 through
+vlfm_gemm_f16_resid_ln with the engine's split-K workspace (stream-K + the LayerNorm launch that reduces it)."""
+import os, sys, subprocess
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
-from vlfm_b200.vlm.dense import gemm_f16
+from vlfm_b200.vlm.dense import gemm_f16, gemm_f16_resid_ln
 
 SHAPES = [(257, 4224, 1408, 0), (257, 1408, 1408, 2), (257, 6144, 1408, 1), (257, 1408, 6144, 2),
           (32, 2304, 768, 0), (32, 768, 768, 2), (32, 3072, 768, 1), (32, 768, 3072, 2), (257, 9216, 1408, 0)]
 N = 200
+PARTIAL_FLOATS = 8 * 257 * 1408      # the BLIP-2 engine's workspace at batch 1 (partials_floats in vlm/blip2_engine.py)
 
-def bench(M, Nn, K, epi):
+def bench(M, Nn, K, epi, resid_ln=False):
     # distinct weights per launch (ring of 8) so that weights stream from HBM like in the real forward
     a = torch.randn(M, K, device="cuda").half()
     ws = [torch.randn(Nn, K, device="cuda").half() for _ in range(8)]
     b = torch.zeros(Nn, device="cuda")
     o = torch.zeros(M, Nn, device="cuda", dtype=torch.float32 if epi >= 2 else torch.float16)
+    if resid_ln:
+        gamma, beta = torch.ones(Nn, device="cuda"), torch.zeros(Nn, device="cuda")
+        y16 = torch.empty(M, Nn, device="cuda", dtype=torch.float16)
+        partials = torch.empty(PARTIAL_FLOATS, device="cuda")
     def seq():
-        for i in range(N): gemm_f16(a, ws[i % 8], b, epi, o)
+        for i in range(N):
+            if resid_ln:
+                gemm_f16_resid_ln(a, ws[i % 8], b, o, gamma, beta, 1e-6, out16=y16, partials=partials)
+            else:
+                gemm_f16(a, ws[i % 8], b, epi, o)
     s = torch.cuda.Stream()
     with torch.cuda.stream(s):
         seq(); torch.cuda.synchronize()
@@ -30,19 +42,28 @@ def bench(M, Nn, K, epi):
         e1.record(); torch.cuda.synchronize()
     return e0.elapsed_time(e1) * 1e3 / (5 * N)
 
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as e:          # the timings stand without it; say that the card was not read
+        q = f"nvidia-smi not readable ({e})"
+    return f"{torch.cuda.get_device_name(0)} | power limit, SM clock, max SM clock: {q}"
+
 sweep = len(sys.argv) > 1 and sys.argv[1] == "sweep"
 vit = 0.0
 for i, (M, Nn, K, epi) in enumerate(SHAPES):
     os.environ.pop("VLFM_GEMM_FORCE", None)
-    base = bench(M, Nn, K, epi)
+    ln = i < 4 and epi == 2
+    base = bench(M, Nn, K, epi, resid_ln=ln)
     vit += base if i < 4 else 0.0
-    line = f"{M}x{Nn}x{K} epi{epi}: model-plan {base:6.2f} us ({2*M*Nn*K/base/1e6:6.1f} TF)"
+    line = f"{M}x{Nn}x{K} epi{epi}{' +LN' if ln else ''}: model-plan {base:6.2f} us ({2*M*Nn*K/base/1e6:6.1f} TF)"
     if sweep:
         for bn in (128, 64, 32):
             for sp in ((1, 2, 3, 4, 6, 8) if epi == 2 else (1,)):
                 os.environ["VLFM_GEMM_FORCE"] = f"{bn}:{sp}"
                 line += f" | {bn}:{sp}={bench(M, Nn, K, epi):.2f}"
     print(line, flush=True)
-# the four ViT-g layer GEMMs at batch 1 (qkv, proj, fc1, fc2) x 39 layers; proj and fc2 run here without a workspace (plain
-# residual epilogue), not through the stream-K path of vlfm_gemm_f16_resid_ln that the forward uses
+# the four ViT-g layer GEMMs at batch 1 (qkv, proj + LayerNorm, fc1, fc2 + LayerNorm) x 39 layers
 print(f"ViT-g batch-1 GEMMs x 39 layers: {vit * 39 / 1e3:.3f} ms", flush=True)
+print(card(), flush=True)

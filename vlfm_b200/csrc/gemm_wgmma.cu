@@ -287,8 +287,11 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       }
     }
   } else if (warp >= 4) {
-    // ---- consumers: warpgroup wg owns rows [64 * wg, +64) of the tile, warp wq of it rows [16 * wq, +16) of those
-    const int wg = (warp >> 2) - 1, wq = warp & 3;
+    // ---- consumers: warpgroup wg owns rows [64 * wg, +64) of the tile, warp wq of it rows [16 * wq, +16) of those.
+    // wg is broadcast from lane 0 so that ptxas can treat it as warp-uniform.  Computed from threadIdx alone, it makes the
+    // `!active` branch below look divergent, and ptxas then serialises every wgmma of the loop (warning C7518): a wait after
+    // each one, so no group stays in flight across K-blocks (DESIGN §3.3).
+    const int wg = __shfl_sync(0xffffffffu, (warp >> 2) - 1, 0), wq = warp & 3;
     const int et = threadIdx.x - (GEMM_THREADS - GEMM_CONSUMERS);
     // a warpgroup whose rows are all past M issues no MMA (a stream-K range may span row tiles: there both always compute)
     const bool active = sk || m_first * BM + wg * 64 < g.M;
