@@ -169,6 +169,16 @@ int vlfm_layernorm_reduce(float* d_x, const float* d_partials, int splits, long 
                           float eps, void* stream);
 int vlfm_gemm_f16(const void* d_A, const void* d_W, const float* d_bias, void* d_out, int M, int N,
                   int K, int lda, int ldw, int ldo, int epilogue, void* stream);
+/* Epilogue flag of vlfm_gemm_f16 (OR it into the epilogue code): the caller allows the batch-1 ViT plan, whose summation order
+ * differs from the plan for other row counts.  At 256 < M <= 258 the GEMM then runs one 256-row tile per column block and splits
+ * K over a thread-block cluster, reduced in shared memory in rank order (bitwise reproducible, no atomics, residual epilogue
+ * included).  Other M, weights below 8 Mi elements (there it measured slower), or VLFM_GEMM_CSPLIT=0 in the environment ignore
+ * it; VLFM_GEMM_CSPLIT=2 takes it for any weight size.  vlfm_gemm_f16_resid_ln takes that plan when it is given a workspace,
+ * and then leaves the workspace untouched.                                                                                    */
+#define VLFM_EPI_CLUSTER_SPLIT 256
+/* The cluster-split plan of an M x N x K GEMM that allows it: tile width *bn, cluster size *splits, and the bytes the busiest CTA
+ * loads (*cta_bytes: K-loop operands plus the peers' partials); all zero when the shape does not take that path.          */
+int vlfm_gemm_csplit_plan(int M, int N, int K, int* bn, int* splits, double* cta_bytes);
 
 /* PIL-exact antialiased bicubic resize (uint8) + ToTensor + Normalize, emitted in the
  * im2col layout of the patch-embedding GEMM.  Replaces lavis' BlipImageEvalProcessor as

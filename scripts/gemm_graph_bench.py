@@ -2,10 +2,13 @@
 (no CPU launch bound), optional sweep of the tile plan via VLFM_GEMM_FORCE=bn:splits.
 
 The four ViT-g layer GEMMs at batch 1 run as the forward runs them: qkv and fc1 through vlfm_gemm_f16, proj and fc2 through
-vlfm_gemm_f16_resid_ln with the engine's split-K workspace (stream-K + the LayerNorm launch that reduces it)."""
-import os, sys, subprocess
+vlfm_gemm_f16_resid_ln with the engine's split-K workspace, and qkv and fc1 with the EPI_CLUSTER_SPLIT flag the engine sets.
+Those four are timed under both batch-1 plans, alternated: the cluster split (one 256-row tile per column block, K split over a
+thread-block cluster) and VLFM_GEMM_CSPLIT=0 (128-row tiles, sub-wave tile widths, stream-K + LayerNorm reduction)."""
+import ctypes, os, sys, subprocess
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
+from vlfm_b200 import _lib
 from vlfm_b200.vlm.dense import gemm_f16, gemm_f16_resid_ln
 
 SHAPES = [(257, 4224, 1408, 0), (257, 1408, 1408, 2), (257, 6144, 1408, 1), (257, 1408, 6144, 2),
@@ -28,7 +31,7 @@ def bench(M, Nn, K, epi, resid_ln=False):
             if resid_ln:
                 gemm_f16_resid_ln(a, ws[i % 8], b, o, gamma, beta, 1e-6, out16=y16, partials=partials)
             else:
-                gemm_f16(a, ws[i % 8], b, epi, o)
+                gemm_f16(a, ws[i % 8], b, epi | _lib.EPI_CLUSTER_SPLIT, o)
     s = torch.cuda.Stream()
     with torch.cuda.stream(s):
         seq(); torch.cuda.synchronize()
@@ -50,12 +53,43 @@ def card():
         q = f"nvidia-smi not readable ({e})"
     return f"{torch.cuda.get_device_name(0)} | power limit, SM clock, max SM clock: {q}"
 
+def csplit_plan(M, Nn, K):
+    """(BN, cluster size, bytes the busiest CTA loads, bytes all CTAs load) of the cluster-split plan, or None."""
+    bn, sp, cta = ctypes.c_int(), ctypes.c_int(), ctypes.c_double()
+    _lib.load().vlfm_gemm_csplit_plan(M, Nn, K, ctypes.addressof(bn), ctypes.addressof(sp), ctypes.addressof(cta))
+    if not bn.value:
+        return None
+    nk = (K + 63) // 64
+    return bn.value, sp.value, cta.value, (Nn + bn.value - 1) // bn.value * nk * (256 + bn.value) * 64 * 2
+
+def with_plan(csplit, fn, *args, **kw):
+    os.environ["VLFM_GEMM_CSPLIT"] = "1" if csplit else "0"
+    try:
+        return fn(*args, **kw)
+    finally:
+        os.environ.pop("VLFM_GEMM_CSPLIT", None)
+
+ROUNDS = 3
 sweep = len(sys.argv) > 1 and sys.argv[1] == "sweep"
 vit = 0.0
+vit_old = 0.0
 for i, (M, Nn, K, epi) in enumerate(SHAPES):
     os.environ.pop("VLFM_GEMM_FORCE", None)
     ln = i < 4 and epi == 2
-    base = bench(M, Nn, K, epi, resid_ln=ln)
+    if i < 4:
+        # old and new plan alternated, ROUNDS times each; the median of each
+        old, new = [], []
+        for _ in range(ROUNDS):
+            old.append(with_plan(False, bench, M, Nn, K, epi, resid_ln=ln))
+            new.append(with_plan(True, bench, M, Nn, K, epi, resid_ln=ln))
+        old_m, base = sorted(old)[ROUNDS // 2], sorted(new)[ROUNDS // 2]
+        vit_old += old_m
+        p = csplit_plan(M, Nn, K)
+        plan = "no cluster-split plan" if p is None else f"BN {p[0]}, cluster {p[1]}: busiest CTA {p[2] / 1e3:.0f} KB, all CTAs {p[3] / 1e6:.1f} MB"
+        print(f"{M}x{Nn}x{K} epi{epi}{' +LN' if ln else ''}: VLFM_GEMM_CSPLIT=0 {' '.join(f'{t:.2f}' for t in old)} us | "
+              f"cluster split {' '.join(f'{t:.2f}' for t in new)} us ({plan})", flush=True)
+    else:
+        base = bench(M, Nn, K, epi, resid_ln=ln)
     vit += base if i < 4 else 0.0
     line = f"{M}x{Nn}x{K} epi{epi}{' +LN' if ln else ''}: model-plan {base:6.2f} us ({2*M*Nn*K/base/1e6:6.1f} TF)"
     if sweep:
@@ -65,5 +99,6 @@ for i, (M, Nn, K, epi) in enumerate(SHAPES):
                 line += f" | {bn}:{sp}={bench(M, Nn, K, epi):.2f}"
     print(line, flush=True)
 # the four ViT-g layer GEMMs at batch 1 (qkv, proj + LayerNorm, fc1, fc2 + LayerNorm) x 39 layers
-print(f"ViT-g batch-1 GEMMs x 39 layers: {vit * 39 / 1e3:.3f} ms", flush=True)
+print(f"ViT-g batch-1 GEMMs x 39 layers (medians): cluster split {vit * 39 / 1e3:.3f} ms, VLFM_GEMM_CSPLIT=0 {vit_old * 39 / 1e3:.3f} ms",
+      flush=True)
 print(card(), flush=True)

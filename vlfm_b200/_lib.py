@@ -17,6 +17,7 @@ ST_FRONTIER_OVERFLOW = 4
 FUSE_WEIGHTED, FUSE_MAX_CONFIDENCE, FUSE_REPLACE, FUSE_EQUAL = 0, 1, 2, 4
 EPI_BIAS_F16, EPI_BIAS_GELU_F16, EPI_BIAS_RESID_F32, EPI_BIAS_F32, EPI_BIAS_RELU_F16 = 0, 1, 2, 3, 4
 EPI_BIAS_GELU_F16X2 = 6
+EPI_CLUSTER_SPLIT = 256      # flag bit of vlfm_gemm_f16's epilogue: the batch-1 ViT cluster-split plan is allowed
 DRAW_LINE, DRAW_CIRCLE, DRAW_RECORD_INTS = 0, 1, 8
 
 
@@ -64,6 +65,7 @@ _SIGNATURES = {
     "vlfm_holes_workspace_bytes": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "vlfm_fill_small_holes": (C.c_int, [_P, C.c_int, C.c_int, C.c_double, _P, _P, _P, _P]),
     "vlfm_gemm_f16": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "vlfm_gemm_csplit_plan": (C.c_int, [C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "vlfm_gemm_f16_resid_ln": (C.c_int, [_P, _P, _P, _P] + [C.c_int] * 6 + [_P, _P, _P, C.c_int, _P, C.c_int, C.c_float, _P, C.c_size_t, _P]),
     "vlfm_layernorm_reduce": (C.c_int, [_P, _P, C.c_int, C.c_longlong, _P, _P, _P, _P] + [C.c_int] * 5 + [C.c_float, _P]),
     "vlfm_preprocess_im2col": (C.c_int, [_P, _P, _P] + [C.c_int] * 7 + [_P, _P, C.c_int, _P, _P, C.c_int,

@@ -428,6 +428,200 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   }
 }
 
+// ================================================================================================
+// Batch-1 ViT GEMMs (256 < M <= 256 + GEMM_TAIL_MAX, the caller allows a cluster split): one 256 x BN tile covers all rows, so
+// every weight byte is delivered to one CTA only, and K is split over the s CTAs of a thread-block cluster.
+//   warpgroup 0     warp 0, one thread: TMA producer (A 256 x 64 and W BN x 64 per stage), as in gemm_f16_wgmma_kernel.
+//   warpgroups 1-4  consumers, 64 rows each (m64nBNk16); the consumer threads of warpgroups 1-2 also compute the tail rows
+//                   (rows 256, 257) on CUDA cores from the swizzled W stages.
+// CTA r of the cluster runs K-blocks [r nk / s, (r + 1) nk / s).  After its slice it stores the fp32 accumulators and tail-row
+// sums into its own shared memory (over the ring), one cluster barrier publishes them, and CTA r reduces rows
+// [r R / s, (r + 1) R / s) of the R = M rows by reading every peer's tile (ld.shared::cluster) in rank order 0..s-1, adds the
+// bias once and runs the epilogue: one writer per element, nothing through global memory, the same bits on every run.
+// A second cluster barrier keeps each CTA's shared memory alive until its peers have read it.  The cluster is touched only
+// after the main loop: the K loop has no cluster-scope barrier.
+// ================================================================================================
+constexpr int CS_BM = 256;
+constexpr int CS_THREADS = 640;      // warpgroup 0 TMA producer, warpgroups 1-4 consumers
+constexpr int CS_CONSUMERS = 512;
+
+__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ uint32_t cluster_nctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ void cluster_sync_all() {
+  __syncwarp();
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ float2 ld_peer_f2(uint32_t saddr, uint32_t rank) {
+  uint32_t a;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(saddr), "r"(rank));
+  float2 v;
+  asm volatile("ld.shared::cluster.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
+  return v;
+}
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(CS_THREADS, 1)
+gemm_f16_csplit_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmArgs g) {
+  constexpr uint32_t A_BYTES = CS_BM * BK * 2, B_BYTES = BN * BK * 2;
+  constexpr int LDP = BN + 8;   // row stride (floats) of the fp32 partial tile: rows 32 bytes apart, conflict-free fragment stores
+  static_assert((size_t)(CS_BM + GEMM_TAIL_MAX) * LDP * 4 <= (size_t)STAGES * (A_BYTES + B_BYTES), "partial tile must fit the ring");
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* sA = smem_align_1024(smem_raw);
+  uint8_t* sB = sA + STAGES * A_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + STAGES * B_BYTES);
+  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + STAGES);
+  float* sbias = reinterpret_cast<float*>(bars + 2 * STAGES);   // [BN]
+  __half* sx = reinterpret_cast<__half*>(sbias + BN);           // the tail rows' K slice
+  float* part = reinterpret_cast<float*>(sA);                    // after the K loop: [CS_BM + tail_rows][LDP] fp32, over the ring
+
+  pdl_trigger();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nk = (g.K + BK - 1) / BK;
+  const int s_cl = (int)cluster_nctarank(), rank = (int)cluster_ctarank();
+  const int n_blk = blockIdx.x / s_cl;
+  const int kb_lo = rank * nk / s_cl, kb_hi = (rank + 1) * nk / s_cl;    // the host plan keeps s <= nk: no slice is empty
+
+  if (warp == 0 && lane == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+    for (int i = 0; i < STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, CS_CONSUMERS / 32); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
+      // weight tiles before the programmatic-dependency wait, activations after it (as in gemm_f16_wgmma_kernel)
+      const int pre = min(kb_hi - kb_lo, STAGES);
+      for (int i = 0; i < pre; ++i) {
+        mbar_expect_tx(full0 + 8 * i, A_BYTES + B_BYTES);
+        tma_load_2d(smem_u32(sB + i * B_BYTES), &tmB, (kb_lo + i) * BK, n_blk * BN, full0 + 8 * i);
+      }
+      pdl_wait();
+      for (int i = 0; i < pre; ++i) tma_load_2d(smem_u32(sA + i * A_BYTES), &tmA, (kb_lo + i) * BK, 0, full0 + 8 * i);
+      int s = pre == STAGES ? 0 : pre; uint32_t ph = pre == STAGES ? 1 : 0;
+      for (int kb = kb_lo + pre; kb < kb_hi; ++kb) {
+        mbar_wait(empty0 + 8 * s, ph ^ 1);
+        mbar_expect_tx(full0 + 8 * s, A_BYTES + B_BYTES);
+        tma_load_2d(smem_u32(sA + s * A_BYTES), &tmA, kb * BK, 0, full0 + 8 * s);
+        tma_load_2d(smem_u32(sB + s * B_BYTES), &tmB, kb * BK, n_blk * BN, full0 + 8 * s);
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+    }
+    __syncwarp();
+  } else {
+    // wg broadcast from lane 0 so that ptxas treats it as warp-uniform (see gemm_f16_wgmma_kernel)
+    const int wg = __shfl_sync(0xffffffffu, (warp >> 2) - 1, 0), wq = warp & 3;
+    const int et = threadIdx.x - (CS_THREADS - CS_CONSUMERS);
+    if (et < BN) { const int n = n_blk * BN + et; sbias[et] = (g.bias && n < g.N) ? __ldg(g.bias + n) : 0.f; }
+    asm volatile("bar.sync 1, 512;" ::: "memory");
+    pdl_wait();
+    // tail rows on CUDA cores: thread = (feature f, K half hk) over the first 2 BN consumer threads
+    const int f = et >> 1, hk = et & 1;
+    float tacc[GEMM_TAIL_MAX];
+#pragma unroll
+    for (int r = 0; r < GEMM_TAIL_MAX; ++r) tacc[r] = 0.f;
+    const int kslice = (kb_hi - kb_lo) * BK, kbase = kb_lo * BK;
+    for (int i = et; i < g.tail_rows * (kslice >> 3); i += CS_CONSUMERS) {
+      const int r = i / (kslice >> 3), c8 = (i - r * (kslice >> 3)) << 3;
+      uint4 xv = make_uint4(0u, 0u, 0u, 0u);
+      if (kbase + c8 < g.K) xv = __ldg(reinterpret_cast<const uint4*>(g.a_tail + (size_t)r * g.lda + kbase + c8));
+      *reinterpret_cast<uint4*>(sx + (size_t)r * kslice + c8) = xv;
+    }
+    asm volatile("bar.sync 1, 512;" ::: "memory");
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int s = 0; uint32_t ph = 0;
+    for (int kb = kb_lo; kb < kb_hi; ++kb) {
+      mbar_wait(full0 + 8 * s, ph);
+      const uint32_t a0 = smem_u32(sA + s * A_BYTES) + (uint32_t)wg * (64 * BK * 2), b0 = smem_u32(sB + s * B_BYTES);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+        Wgmma<BN>::mma(acc, wgmma_desc_k128(a0 + k * 32), wgmma_desc_k128(b0 + k * 32), (kb > kb_lo || k > 0) ? 1u : 0u);
+      wg_commit();
+      if (f < BN) {     // overlaps the MMAs just issued
+        const uint8_t* wrow = sB + (size_t)s * B_BYTES + (size_t)f * 128;
+        const int k0 = (kb - kb_lo) * BK + hk * 32;
+        // one 16-byte W chunk at a time (registers: the 64 accumulators of BN 128 share 96 per thread); per row the FMA chain
+        // runs over c, e in the same order as in gemm_f16_wgmma_kernel
+        float a[GEMM_TAIL_MAX];
+#pragma unroll
+        for (int r = 0; r < GEMM_TAIL_MAX; ++r) a[r] = 0.f;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const uint4 wv = *reinterpret_cast<const uint4*>(wrow + (((hk * 4 + c) ^ (f & 7)) << 4));
+          const __half2* wh = reinterpret_cast<const __half2*>(&wv);
+#pragma unroll
+          for (int r = 0; r < GEMM_TAIL_MAX; ++r) {
+            if (r < g.tail_rows) {
+              const uint4 xv = *reinterpret_cast<const uint4*>(sx + (size_t)r * kslice + k0 + c * 8);
+              const __half2* xh = reinterpret_cast<const __half2*>(&xv);
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const float2 xf = __half22float2(xh[e]), wf = __half22float2(wh[e]);
+                a[r] = fmaf(xf.x, wf.x, a[r]); a[r] = fmaf(xf.y, wf.y, a[r]);
+              }
+            }
+          }
+        }
+#pragma unroll
+        for (int r = 0; r < GEMM_TAIL_MAX; ++r) tacc[r] += a[r];
+      }
+      wg_wait<1>();
+      if (kb > kb_lo) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty0 + 8 * (s == 0 ? STAGES - 1 : s - 1));
+      }
+      if (++s == STAGES) { s = 0; ph ^= 1; }
+    }
+    wg_wait<0>();
+#pragma unroll
+    for (int r = 0; r < GEMM_TAIL_MAX; ++r) tacc[r] += __shfl_xor_sync(0xffffffffu, tacc[r], 1);
+    if (s_cl == 1) {
+      // unsplit: the epilogue straight from the fragments
+      if (hk == 0 && f < BN && n_blk * BN + f < g.N) {
+#pragma unroll
+        for (int r = 0; r < GEMM_TAIL_MAX; ++r)
+          if (r < g.tail_rows) epilogue_store2(g, CS_BM + r, n_blk * BN + f, tacc[r] + sbias[f], 0.f, false, false);
+      }
+      epilogue_frag<BN>(acc, wg * 64 + wq * 16, n_blk, g, false, true, sbias);
+    } else {
+      asm volatile("bar.sync 1, 512;" ::: "memory");     // every warpgroup has finished reading the ring
+      const int r_up = wg * 64 + wq * 16 + (lane >> 2), cq = (lane & 3) * 2;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        *reinterpret_cast<float2*>(part + r_up * LDP + j * 8 + cq) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(part + (r_up + 8) * LDP + j * 8 + cq) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      if (hk == 0 && f < BN) {
+#pragma unroll
+        for (int r = 0; r < GEMM_TAIL_MAX; ++r)
+          if (r < g.tail_rows) part[(CS_BM + r) * LDP + f] = tacc[r];
+      }
+    }
+  }
+  if (s_cl > 1) {
+    cluster_sync_all();           // every CTA's partial tile is visible to the cluster
+    if (warp >= 4) {
+      const int et = threadIdx.x - (CS_THREADS - CS_CONSUMERS);
+      const int rows = CS_BM + g.tail_rows, r0 = rank * rows / s_cl, r1 = (rank + 1) * rows / s_cl;
+      const uint32_t base = smem_u32(part);
+      for (int i = et; i < (r1 - r0) * (BN / 2); i += CS_CONSUMERS) {
+        const int row = r0 + i / (BN / 2), c = (i % (BN / 2)) * 2, n = n_blk * BN + c;
+        if (n >= g.N) continue;
+        const uint32_t off = base + (uint32_t)(row * LDP + c) * 4;
+        float2 sum = ld_peer_f2(off, 0);
+        for (int p = 1; p < s_cl; ++p) { const float2 v = ld_peer_f2(off, p); sum.x += v.x; sum.y += v.y; }
+        epilogue_store2(g, row, n, sum.x + sbias[c], sum.y + sbias[c + 1], n + 1 < g.N, false);
+      }
+    }
+    cluster_sync_all();           // no CTA exits while a peer may still read its shared memory
+  }
+}
 
 // ================================================================================================
 // "x2" GEMM: fp32-grade product on the fp16 tensor path (the Q-Former, which the reference runs in float32).
@@ -628,12 +822,62 @@ static int launch_gemm_x2(const CUtensorMap& ta, const CUtensorMap& tal, const v
   return VLFM_OK;
 }
 
+// gemm_f16_csplit_wgmma_kernel<BN, STAGES>: its shared memory, how many s-CTA clusters of it the device runs at once, and the
+// launch (grid of column tiles x s, cluster (s, 1, 1), programmatic dependent launch as for the other kernels)
+template <int BN, int STAGES>
+struct Csplit {
+  static constexpr size_t smem = (size_t)STAGES * (CS_BM * BK * 2 + BN * BK * 2) + 2 * STAGES * 8 + 1024 + BN * 4 +
+                                 (size_t)GEMM_TAIL_MAX * GEMM_TAIL_KMAX * 2;
+  static_assert(smem <= 227 * 1024, "cluster-split GEMM stage ring exceeds the 227 KB a block may use");
+  static int configure() {
+    static int rc = -1;
+    if (rc < 0) rc = check_cuda(cudaFuncSetAttribute(gemm_f16_csplit_wgmma_kernel<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                                "cudaFuncSetAttribute(gemm csplit)");
+    return rc;
+  }
+  static int max_clusters(int s) {
+    static int fit[9] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};
+    if (fit[s] < 0) {
+      fit[s] = 0;
+      if (configure()) return 0;
+      cudaLaunchConfig_t cfg{};
+      cfg.gridDim = dim3(s); cfg.blockDim = dim3(CS_THREADS); cfg.dynamicSmemBytes = smem;
+      cudaLaunchAttribute attr[1];
+      attr[0].id = cudaLaunchAttributeClusterDimension;
+      attr[0].val.clusterDim.x = s; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+      cfg.attrs = attr; cfg.numAttrs = 1;
+      int n = 0;
+      if (cudaOccupancyMaxActiveClusters(&n, gemm_f16_csplit_wgmma_kernel<BN, STAGES>, &cfg) == cudaSuccess) fit[s] = n;
+      else cudaGetLastError();
+    }
+    return fit[s];
+  }
+  static int launch(const CUtensorMap& ta, const void* W, int ldw, const GemmArgs& g, int s, cudaStream_t st) {
+    CUtensorMap tb;
+    int rc = make_map(&tb, W, g.N, g.K, ldw, BN);
+    if (!rc) rc = configure();
+    if (rc) return rc;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(((g.N + BN - 1) / BN) * s); cfg.blockDim = dim3(CS_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = s; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 2 : 1;
+    rc = check_cuda(cudaLaunchKernelEx(&cfg, gemm_f16_csplit_wgmma_kernel<BN, STAGES>, ta, tb, g), "gemm_f16_csplit_wgmma_kernel");
+    if (rc) return rc;
+    count_launch();
+    return VLFM_OK;
+  }
+};
+
 }  // namespace vlfm
 
 using namespace vlfm;
 
 static int gemm_dispatch(const void* d_A, const void* d_W, int M, int N, int K, int lda, int ldw, GemmArgs g, void* stream, float* d_partials,
-                         size_t partial_bytes, SplitK* layout);
+                         size_t partial_bytes, SplitK* layout, bool csplit);
 
 // SMs of the current device (one GEMM CTA per SM): the launch plans size a wave by it.  132 on an H100 SXM.
 static int sm_count() {
@@ -647,9 +891,59 @@ extern "C" int vlfm_gemm_f16(const void* d_A, const void* d_W, const float* d_bi
   if (!d_A || !d_W || !d_out || M < 1 || N < 1 || K < 1) { set_error("vlfm_gemm_f16: bad argument"); return VLFM_E_INVALID; }
   if ((K & 7) || (lda & 7) || (ldw & 7) || (ldo & 7) || ((uintptr_t)d_A & 15) || ((uintptr_t)d_W & 15) || ((uintptr_t)d_out & 15)) {
     set_error("vlfm_gemm_f16: K, lda, ldw, ldo must be multiples of 8 and pointers 16-byte aligned"); return VLFM_E_INVALID; }
+  const bool csplit = (epilogue & VLFM_EPI_CLUSTER_SPLIT) != 0;
+  epilogue &= ~VLFM_EPI_CLUSTER_SPLIT;
   if (epilogue < 0 || epilogue > 4) { set_error("vlfm_gemm_f16: unknown epilogue %d", epilogue); return VLFM_E_INVALID; }
   GemmArgs g{d_bias, d_out, M, N, K, ldo, epilogue, (K + BK - 1) / BK, 0, nullptr, 0, 0, 0, nullptr, BM};
-  return gemm_dispatch(d_A, d_W, M, N, K, lda, ldw, g, stream, nullptr, 0, nullptr);
+  return gemm_dispatch(d_A, d_W, M, N, K, lda, ldw, g, stream, nullptr, 0, nullptr, csplit);
+}
+
+// Cluster-split plan (gemm_f16_csplit_wgmma_kernel) for 256 < M <= 256 + GEMM_TAIL_MAX.  Over the tile widths BN and cluster
+// sizes s whose clusters all run at once (cudaOccupancyMaxActiveClusters: the GPCs do not split evenly into clusters), the one
+// that minimises what the busiest CTA takes in: its K-blocks x (256 + BN) x 64 fp16, plus, when split, the peers' fp32 partials
+// its reduction reads ((s - 1) / s of an M x BN tile) and a fixed cost per cluster reduction.  A byte model, not a fitted one.
+constexpr double CS_RED_FIXED_BYTES = 16384;   // the two cluster barriers and the reduction's latency, counted as K-loop bytes
+// Which shapes take it.  On an H100 (DESIGN §3.3) the plan below is faster than the 128-row plan for the ViT's fc1 and fc2
+// (8.7 M weights each) and slower for qkv (5.9 M) and proj (2.0 M), whose shorter K loops do not pay back the cluster launch
+// and the reduction.  So by default it runs for weights of at least CS_MIN_WEIGHTS elements.  VLFM_GEMM_CSPLIT=0 turns it off,
+// =2 runs it for every shape it can take (tests, sweeps).
+constexpr long long CS_MIN_WEIGHTS = 8ll << 20;
+static bool csplit_eligible(int M, int N, int K) {
+  const char* e = getenv("VLFM_GEMM_CSPLIT");
+  const int mode = (e && e[0]) ? atoi(e) : 1;
+  return mode > 0 && M > CS_BM && M - CS_BM <= GEMM_TAIL_MAX && K <= GEMM_TAIL_KMAX && (mode >= 2 || (long long)N * K >= CS_MIN_WEIGHTS);
+}
+struct CsplitPlan { int bn, s; double cta_bytes; };
+static int csplit_fit(int bn, int s) {
+  if (bn == 128) return Csplit<128, 4>::max_clusters(s);
+  if (bn == 96) return Csplit<96, 4>::max_clusters(s);
+  return Csplit<64, 5>::max_clusters(s);
+}
+static CsplitPlan csplit_plan(int M, int N, int K) {
+  const int nk = (K + BK - 1) / BK;
+  CsplitPlan best{0, 0, 0.0};
+  const int bns[3] = {128, 96, 64};
+  for (int bn : bns) {
+    const int nt = (N + bn - 1) / bn;
+    for (int s = 1; s <= 8 && s <= nk; ++s) {
+      if (nt > csplit_fit(bn, s)) continue;
+      double bytes = (double)((nk + s - 1) / s) * (CS_BM + bn) * BK * 2;
+      if (s > 1) bytes += (double)(s - 1) / s * M * bn * 4 + CS_RED_FIXED_BYTES;
+      if (!best.bn || bytes < best.cta_bytes) best = CsplitPlan{bn, s, bytes};
+    }
+  }
+  return best;
+}
+
+// The plan vlfm_gemm_f16 / vlfm_gemm_f16_resid_ln would run for an allowed cluster split of this shape: {BN, s, bytes the busiest
+// CTA loads}, or {0, 0, 0} when the shape does not take that path.  For scripts/gemm_graph_bench.py.
+extern "C" int vlfm_gemm_csplit_plan(int M, int N, int K, int* bn, int* splits, double* cta_bytes) {
+  CsplitPlan p{0, 0, 0.0};
+  if (csplit_eligible(M, N, K)) p = csplit_plan(M, N, K);
+  if (bn) *bn = p.bn;
+  if (splits) *splits = p.s;
+  if (cta_bytes) *cta_bytes = p.cta_bytes;
+  return VLFM_OK;
 }
 
 // Stream-K: the least number of K-blocks a CTA works through.  Below it the fixed cost of a CTA (barrier set-up, the first
@@ -657,10 +951,24 @@ extern "C" int vlfm_gemm_f16(const void* d_A, const void* d_W, const float* d_bi
 constexpr int SK_MIN_ITERS = 3;
 
 static int gemm_dispatch(const void* d_A, const void* d_W, int M, int N, int K, int lda, int ldw, GemmArgs g, void* stream, float* d_partials,
-                         size_t partial_bytes, SplitK* layout) {
+                         size_t partial_bytes, SplitK* layout, bool csplit) {
   if (layout) *layout = SplitK{1, 0};
   const int epilogue = g.epi;
   CUtensorMap ta;
+  // Batch-1 ViT rows (256 < M <= 256 + GEMM_TAIL_MAX) when the caller allows a split whose bits depend on the plan: one 256-row
+  // tile per column block, K split over a thread-block cluster and reduced in shared memory (csplit_eligible: which shapes).
+  if (csplit && !getenv("VLFM_GEMM_FORCE") && csplit_eligible(M, N, K)) {
+    const CsplitPlan p = csplit_plan(M, N, K);
+    if (p.bn) {
+      int rc = make_map(&ta, d_A, M, K, lda, CS_BM);
+      if (rc) return rc;
+      g.a_tail = (const __half*)d_A + (size_t)CS_BM * lda; g.lda = lda; g.tail_rows = M - CS_BM; g.tail_row0 = CS_BM;
+      cudaStream_t cst = (cudaStream_t)stream;
+      if (p.bn == 128) return Csplit<128, 4>::launch(ta, d_W, ldw, g, p.s, cst);
+      if (p.bn == 96) return Csplit<96, 4>::launch(ta, d_W, ldw, g, p.s, cst);
+      return Csplit<64, 5>::launch(ta, d_W, ldw, g, p.s, cst);
+    }
+  }
   g.a_box_rows = M <= 32 ? 32 : (M <= 64 ? 64 : BM);
   int rc = make_map(&ta, d_A, M, K, lda, g.a_box_rows);
   if (rc) return rc;
@@ -790,7 +1098,9 @@ extern "C" int vlfm_gemm_f16_resid_ln(const void* d_A, const void* d_W, const fl
       ((uintptr_t)d_x & 15) || ((uintptr_t)d_partials & 15)) { set_error("vlfm_gemm_f16_resid_ln: alignment (K, strides %% 8; N %% 4; 16-byte pointers)"); return VLFM_E_INVALID; }
   GemmArgs g{d_bias, d_x, M, N, K, ldx, VLFM_EPI_BIAS_RESID_F32, (K + BK - 1) / BK, 0, nullptr, 0, 0, 0, nullptr, BM};
   SplitK layout;
-  int rc = gemm_dispatch(d_A, d_W, M, N, K, lda, ldw, g, stream, d_partials, partial_bytes, &layout);
+  // a workspace means the caller allows a split K, which includes the cluster split (MobileSAM passes none: its rows' bits must
+  // not depend on M)
+  int rc = gemm_dispatch(d_A, d_W, M, N, K, lda, ldw, g, stream, d_partials, partial_bytes, &layout, d_partials != nullptr);
   if (rc) return rc;
   if (layout.splits != 1) return layernorm_reduce_impl(d_x, d_partials, layout, d_gamma, d_beta, d_out16, nullptr, d_out32, M, N, ldx, ld16, ld32, eps, stream);
   return vlfm_layernorm(d_x, d_gamma, d_beta, d_out16, d_out32, M, N, ldx, ld16, ld32, eps, stream);

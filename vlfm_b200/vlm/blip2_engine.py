@@ -174,9 +174,10 @@ class Blip2ITCEngine:
 
     # ---------------------------------------------------------------- primitives ----
     # _gemm / _gemm_x2 stay methods: bench.py's GEMM replay swaps them for recording wrappers (with fuse_ln off, every GEMM of the
-    # forward goes through them)
+    # forward goes through them).  The ViT's GEMMs allow the batch-1 cluster-split plan (257 rows: one 256-row tile per column
+    # block, K split over a thread-block cluster); its rows' bits depend on that plan, which only batch 1 runs.
     def _gemm(self, a, w, bias, epi, out):
-        dense.gemm_f16(a, w, bias, epi, out)
+        dense.gemm_f16(a, w, bias, epi | _lib.EPI_CLUSTER_SPLIT, out)
 
     def _gemm_x2(self, a, al, w, wl, bias, epi, out, out_lo=None):
         dense.gemm_f16x2(a, al, w, wl, bias, epi, out, out_lo)

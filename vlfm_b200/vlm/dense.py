@@ -23,13 +23,15 @@ Tensor = torch.Tensor
 
 def gemm_f16(a: Tensor, w: Tensor, bias: Optional[Tensor], epilogue: int, out: Optional[Tensor] = None,
              rows: Optional[int] = None) -> Tensor:
-    """out = epilogue(a[M,K] @ w[N,K]^T + bias).  For EPI_BIAS_RESID_F32 ``out`` is the fp32 residual stream updated in place."""
+    """out = epilogue(a[M,K] @ w[N,K]^T + bias).  For EPI_BIAS_RESID_F32 ``out`` is the fp32 residual stream updated in place.
+    ``epilogue`` may carry the EPI_CLUSTER_SPLIT flag (the batch-1 ViT plan is allowed)."""
     M, K = a.shape
     if rows is not None:
         M = rows
     if out is None:
-        assert epilogue != _lib.EPI_BIAS_RESID_F32, "the residual epilogue updates a caller-given stream"
-        out = torch.empty((M, w.shape[0]), dtype=F32 if epilogue == _lib.EPI_BIAS_F32 else F16, device=a.device)
+        epi = epilogue & ~_lib.EPI_CLUSTER_SPLIT
+        assert epi != _lib.EPI_BIAS_RESID_F32, "the residual epilogue updates a caller-given stream"
+        out = torch.empty((M, w.shape[0]), dtype=F32 if epi == _lib.EPI_BIAS_F32 else F16, device=a.device)
     rc = _lib.load().vlfm_gemm_f16(a.data_ptr(), w.data_ptr(), _lib.ptr(bias), out.data_ptr(), M, w.shape[0], K, a.stride(0),
                                    w.stride(0), out.stride(0), epilogue, _lib.stream_ptr())
     _lib.check(rc, "vlfm_gemm_f16")
