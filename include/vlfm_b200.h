@@ -456,6 +456,52 @@ int vlfm_sam_pixel_shuffle2(const float* d_in, float* d_out, int B, int h, int w
 int vlfm_sam_mask_logits(const float* d_up, const float* d_hyper, float* d_logits, int M, int h, int w, int C, void* stream);
 int vlfm_sam_mask_finish(const float* d_low, uint8_t* d_out, int M, int L, int S, int newh, int neww, int H, int W, void* stream);
 
+/* ------------------------------------------------------------------ PointNav ---- */
+/* Replaces WrappedPointNavResNetPolicy.act (vlfm/policy/utils/pointnav_policy.py:51-128): the ResNet-18 depth encoder with
+ * GroupNorm and the 2-layer LSTM of 512 (engine: vlfm_b200/policy/pointnav_engine.py).  Activations are NHWC.  Each conv is an
+ * im2col pass (vlfm_pointnav_depth_in, vlfm_sam_im2col3x3, vlfm_pointnav_gather_s2) plus vlfm_gemm_f16 with VLFM_EPI_BIAS_F32;
+ * these are the rest.  Every reduction has a fixed order: bitwise reproducible, and independent of the other environments.
+ *
+ * vlfm_pointnav_depth_in: d_depth [B,H,W] fp32 -> torch "area" resize to (IH, IW) (adaptive average pooling, fp32) -> 2x2
+ *   average pool -> the rows of the 7x7 stride-2 pad-3 conv: d_col16 [B*OH*OW, ldk] fp16, column ky*7 + kx, columns >= 49 zero,
+ *   OH = (IH/2 - 1)/2 + 1 (OW likewise).  d_resized [B,IH,IW] fp32 (may be NULL): the resized frame.  (H, W) == (IH, IW) is the
+ *   identity resize, exact.
+ * vlfm_pointnav_groupnorm: GroupNorm(G) statistics per (image, group) of d_x [B,HW,C] fp32 (biased variance, eps inside the
+ *   square root), then out = act(GN_a(x) + r) -> d_out32 (may alias d_r) and / or d_out16.  rmode 0: r = 0; 1: r = d_r (fp32
+ *   [B,HW,C]); 2: r = GN_b(d_y) (the downsample branch, its own statistics).  act = ReLU when relu != 0.
+ * vlfm_pointnav_maxpool3s2: 3x3 stride-2 pad-1 max pool (padding is -inf) of d_x [B,H,W,C] fp32 -> d_out32 and / or d_out16.
+ * vlfm_pointnav_gather_s2: the rows of a 1x1 stride-2 conv: d_out16 [B*Ho*Wo, C] = d_x16 [B, 2yo, 2xo, :] fp16, C % 8 == 0.
+ * vlfm_pointnav_gemv_f32: d_y[b*ldy + n] = act(sum_k d_x[b*ldx + k] d_W[n*ldw + k] + d_bias[n]) in fp32 on CUDA cores, B <= 64;
+ *   W is read once for all B.  Each (b, n) is summed in an order that depends on K only (bitwise the same for any B).
+ *   K, ldx, ldw multiples of 4; d_x, d_W 16-byte aligned; d_bias may be NULL.
+ * vlfm_pointnav_lstm_prep: per environment b (state slot e = d_env_ids[b]; d_state [E,4,512] = [h_l0, h_l1, c_l0, c_l1]), with
+ *   the state zeroed where d_masks[b] == 0: d_xin0 [B,1088] columns 512..543 = tgt_embeding(rho, cos(-theta), sin(-theta)) of
+ *   d_goal [B,2]; 544..575 = the previous-action embedding (discrete: d_w_prev [5,32] row (mask ? d_prev[e] + 1 : 0), d_prev
+ *   int64 [E]; else d_w_prev [32,2] @ (mask * d_prev[e]) + d_b_prev, d_prev fp32 [E,2]); 576.. = h_l0.  d_xin1 [B,1024]
+ *   columns 512.. = h_l1; d_cbuf [B,1024] = [c_l0, c_l1].  (Columns 0..511 of d_xin0 are visual_fc's output.)
+ * vlfm_pointnav_lstm_cell: layer 0 from d_gates [B,2048] (i, f, g, o; both biases included): c_l0' -> d_cbuf[:, :512],
+ *   h_l0' -> d_xin1[:, :512].
+ * vlfm_pointnav_lstm_head: layer 1 from d_gates, then the head d_w_head [4,512] + d_b_head: d_head [B,4] (may be NULL) the four
+ *   outputs (logits; or mu | log_std), d_action the action (discrete: argmax, first index on ties, int64 [B]; else tanh(mu),
+ *   fp32 [B,2]), also stored to d_prev[e]; d_feat [B,512] (may be NULL) = h_l1'; d_state[e] = [h_l0', h_l1', c_l0', c_l1'].
+ *   d_env_ids must not repeat. */
+int vlfm_pointnav_depth_in(const float* d_depth, int B, int H, int W, int IH, int IW, void* d_col16, int ldk, float* d_resized,
+                           void* stream);
+int vlfm_pointnav_groupnorm(const float* d_x, const float* d_gamma_a, const float* d_beta_a, int rmode, const float* d_r,
+                            const float* d_y, const float* d_gamma_b, const float* d_beta_b, float* d_out32, void* d_out16, int B, int HW,
+                            int C, int G, float eps, int relu, void* stream);
+int vlfm_pointnav_maxpool3s2(const float* d_x, float* d_out32, void* d_out16, int B, int H, int W, int C, void* stream);
+int vlfm_pointnav_gather_s2(const void* d_x16, void* d_out16, int B, int H, int W, int C, void* stream);
+int vlfm_pointnav_gemv_f32(const float* d_x, int ldx, const float* d_W, int ldw, const float* d_bias, float* d_y, int ldy, int B, int N,
+                           int K, int relu, void* stream);
+int vlfm_pointnav_lstm_prep(const int32_t* d_env_ids, const float* d_state, const void* d_prev, int discrete, const uint8_t* d_masks,
+                            const float* d_goal, const float* d_w_goal, const float* d_b_goal, const float* d_w_prev,
+                            const float* d_b_prev, float* d_xin0, float* d_xin1, float* d_cbuf, int B, void* stream);
+int vlfm_pointnav_lstm_cell(const float* d_gates, float* d_cbuf, float* d_xin1, int B, void* stream);
+int vlfm_pointnav_lstm_head(const float* d_gates, const float* d_cbuf, const float* d_xin1, const float* d_w_head, const float* d_b_head,
+                            int discrete, const int32_t* d_env_ids, float* d_state, void* d_prev, float* d_feat, float* d_head,
+                            void* d_action, int B, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

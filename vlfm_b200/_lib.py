@@ -123,6 +123,14 @@ _SIGNATURES = {
     "vlfm_sam_pixel_shuffle2": (C.c_int, [_P, _P] + [C.c_int] * 4 + [_P]),
     "vlfm_sam_mask_logits": (C.c_int, [_P, _P, _P] + [C.c_int] * 4 + [_P]),
     "vlfm_sam_mask_finish": (C.c_int, [_P, _P] + [C.c_int] * 7 + [_P]),
+    "vlfm_pointnav_depth_in": (C.c_int, [_P] + [C.c_int] * 5 + [_P, C.c_int, _P, _P]),
+    "vlfm_pointnav_groupnorm": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, _P, _P] + [C.c_int] * 4 + [C.c_float, C.c_int, _P]),
+    "vlfm_pointnav_maxpool3s2": (C.c_int, [_P, _P, _P] + [C.c_int] * 4 + [_P]),
+    "vlfm_pointnav_gather_s2": (C.c_int, [_P, _P] + [C.c_int] * 4 + [_P]),
+    "vlfm_pointnav_gemv_f32": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P] + [C.c_int] * 5 + [_P]),
+    "vlfm_pointnav_lstm_prep": (C.c_int, [_P, _P, _P, C.c_int] + [_P] * 9 + [C.c_int, _P]),
+    "vlfm_pointnav_lstm_cell": (C.c_int, [_P, _P, _P, C.c_int, _P]),
+    "vlfm_pointnav_lstm_head": (C.c_int, [_P] * 5 + [C.c_int] + [_P] * 6 + [C.c_int, _P]),
 }
 
 _lib = None
