@@ -211,6 +211,8 @@ int vlfm_attention_f16(const void* d_q, const void* d_k, const void* d_v, void* 
  * vlfm_attention_f32: softmax(scale * Q K^T) V in float32 (q, k, v fp32; hd in {32, 64}; Nk <= 272), output as x2 operands.
  * vlfm_split_x2: x2 operands of an fp32 array (d_hi may be NULL when the fp16 rounding already exists). */
 #define VLFM_EPI_BIAS_GELU_F16X2 6
+/* vlfm_gemm_f16 only: bias + SiLU (x / (1 + exp(-x)) in fp32) -> fp16 out (YOLOv7 convs with the BatchNorm folded into the bias) */
+#define VLFM_EPI_BIAS_SILU_F16 7
 int vlfm_gemm_f16x2(const void* d_A_hi, const void* d_A_lo, const void* d_W_hi, const void* d_W_lo, const float* d_bias, void* d_out,
                     void* d_out_lo, int M, int N, int K, int lda, int ldw, int ldo, int epilogue, void* stream);
 int vlfm_gemm_f16x2_resid_ln(const void* d_A_hi, const void* d_A_lo, const void* d_W_hi, const void* d_W_lo, const float* d_bias,
@@ -501,6 +503,52 @@ int vlfm_pointnav_lstm_cell(const float* d_gates, float* d_cbuf, float* d_xin1, 
 int vlfm_pointnav_lstm_head(const float* d_gates, const float* d_cbuf, const float* d_xin1, const float* d_w_head, const float* d_b_head,
                             int discrete, const int32_t* d_env_ids, float* d_state, void* d_prev, float* d_feat, float* d_head,
                             void* d_action, int B, void* stream);
+
+/* ------------------------------------------------------------------ YOLOv7 ---- */
+/* Replaces YOLOv7.predict (vlfm/vlm/yolov7.py:50-110): YOLOv7-E6E in fp16 plus yolov7's non_max_suppression and scale_coords
+ * (engine: vlfm_b200/vlm/yolov7_engine.py).  Activations are fp16 NHWC rows with a row stride ld* (elements), so a layer may read
+ * or write one channel slice of a concat buffer.  1x1 convs are vlfm_gemm_f16 on the rows, 3x3 convs vlfm_yolo_im2col3x3 plus
+ * vlfm_gemm_f16, both with VLFM_EPI_BIAS_SILU_F16; these are the rest.  Results are bitwise reproducible.
+ *
+ * vlfm_yolo_preprocess: cv2.resize(INTER_AREA) of d_img [B,H,W,3] uint8 to (OH, OW) (H >= OH, W >= OW; cv2's area tables in CSR
+ *   form, built on the host by vlm/yolov7_engine.py: per destination row dy the entries d_yofs[dy]..d_yofs[dy+1] of (d_ysi, d_ybeta),
+ *   per destination column likewise), fp16(v / 255), then ReOrg: d_out16 [B, OH/2, OW/2, 16], channel g*3 + c with g = (y & 1) +
+ *   2 * (x & 1), channels 12..15 zero.
+ * vlfm_yolo_im2col3x3: d_x16 [B,H,W,C] (row stride ldx) -> d_col16 [B*Ho*Wo, ldk] rows of a 3x3 conv, pad 1, stride 1 or 2, column
+ *   (ky*3+kx)*C + c, columns >= 9C zero.  C, ldx, ldk multiples of 8.
+ * vlfm_yolo_maxpool2: MaxPool2d(2, 2) [B,H,W,C] (ldx) -> [B,H/2,W/2,C] (ldo).
+ * vlfm_yolo_spp_pools: MaxPool2d(k, 1, k/2) for k = 5, 9, 13 of [B,H,W,C] (ldx) -> d_out16 + j*C (ldo) for the j-th.
+ * vlfm_yolo_upsample2: nearest x2 [B,H,W,C] (ldx) -> [B,2H,2W,C] (ldo); C, ldx, ldo multiples of 8.
+ * vlfm_yolo_add: d_out16 = fp16(a + b) over [rows, C] (strides lda, ldb, ldo).
+ * vlfm_yolo_decode: one IDetect level, d_head16 [B,ny,nx,ldh] fp16 (ldh >= na*(nc+5), channel a*(nc+5) + k) -> the frame's candidate rows (level, anchor, y, x) from
+ *   row0: sigmoid, xy = (2s - 0.5 + grid) * stride, wh = (2s)^2 * d_anchors[a] (pixels); a row is kept when obj > conf_thres,
+ *   conf = max_j(cls_j * obj) > conf_thres (first j on ties) and class j is set in class_mask.  Kept rows are appended to
+ *   d_cand [B, R, 8] = [x1, y1, x2, y2, conf, class, row, 0]; d_count [B] counts them (zero it before the first level).
+ * vlfm_yolo_sort: d_order [B, R]: the candidate slots by descending conf, then ascending row.
+ * vlfm_yolo_nms: greedy NMS in that order on the boxes offset by class * 4096 (0 when agnostic), IoU > iou_thres suppresses
+ *   (torchvision.ops.nms), at most max_det keeps: d_keep [B, max_det] candidate slots, d_nkeep [B].
+ * vlfm_yolo_boxes: scale_coords + clip + round + normalise of the kept boxes: (v - pad) / gain clamped to [0, W] (x) or [0, H] (y),
+ *   rounded half to even, / W or / H -> d_boxes [B, max_det, 4], d_scores, d_classes (rows past the count: 0, 0, -1), d_counts [B]. */
+typedef struct VlfmYoloParams {
+  float conf_thres, iou_thres;
+  int32_t agnostic, pad;
+  uint32_t class_mask[4];     /* bit j: class j may be kept */
+} VlfmYoloParams;
+int vlfm_yolo_preprocess(const uint8_t* d_img, void* d_out16, int B, int H, int W, int OH, int OW, const int32_t* d_yofs,
+                         const int32_t* d_ysi, const float* d_ybeta, const int32_t* d_xofs, const int32_t* d_xsi, const float* d_xalpha,
+                         void* stream);
+int vlfm_yolo_im2col3x3(const void* d_x16, int ldx, void* d_col16, int B, int H, int W, int C, int stride, int ldk, void* stream);
+int vlfm_yolo_maxpool2(const void* d_x16, int ldx, void* d_out16, int ldo, int B, int H, int W, int C, void* stream);
+int vlfm_yolo_spp_pools(const void* d_x16, int ldx, void* d_out16, int ldo, int B, int H, int W, int C, void* stream);
+int vlfm_yolo_upsample2(const void* d_x16, int ldx, void* d_out16, int ldo, int B, int H, int W, int C, void* stream);
+int vlfm_yolo_add(const void* d_a16, int lda, const void* d_b16, int ldb, void* d_out16, int ldo, long long rows, int C, void* stream);
+int vlfm_yolo_decode(const void* d_head16, int ldh, int B, int ny, int nx, int na, int nc, const float* d_anchors, float stride, int row0, int R,
+                     const VlfmYoloParams* d_params, float* d_cand, int* d_count, void* stream);
+int vlfm_yolo_sort(const float* d_cand, const int* d_count, int R, int B, int32_t* d_order, void* stream);
+int vlfm_yolo_nms(const float* d_cand, const int32_t* d_order, const int* d_count, int R, int B, const VlfmYoloParams* d_params, int max_det,
+                  int32_t* d_keep, int* d_nkeep, void* stream);
+int vlfm_yolo_boxes(const float* d_cand, const int32_t* d_keep, const int* d_nkeep, int R, int B, int max_det, float gain, float padx,
+                    float pady, int H, int W, float* d_boxes, float* d_scores, int32_t* d_classes, int* d_counts, void* stream);
 
 #ifdef __cplusplus
 }

@@ -17,6 +17,7 @@ ST_FRONTIER_OVERFLOW = 4
 FUSE_WEIGHTED, FUSE_MAX_CONFIDENCE, FUSE_REPLACE, FUSE_EQUAL = 0, 1, 2, 4
 EPI_BIAS_F16, EPI_BIAS_GELU_F16, EPI_BIAS_RESID_F32, EPI_BIAS_F32, EPI_BIAS_RELU_F16 = 0, 1, 2, 3, 4
 EPI_BIAS_GELU_F16X2 = 6
+EPI_BIAS_SILU_F16 = 7
 EPI_CLUSTER_SPLIT = 256      # flag bit of vlfm_gemm_f16's epilogue: the batch-1 ViT cluster-split plan is allowed
 DRAW_LINE, DRAW_CIRCLE, DRAW_RECORD_INTS = 0, 1, 8
 
@@ -44,6 +45,12 @@ class ExploreEnv(C.Structure):
         ("slot", C.c_int32), ("agent_col", C.c_int32), ("agent_row", C.c_int32), ("frame", C.c_int32 * 4), ("pad", C.c_int32),
         ("heading_deg", C.c_double), ("fov_deg", C.c_double), ("max_line_len", C.c_double), ("area_thresh_px", C.c_double),
     ]
+
+
+class YoloParams(C.Structure):
+    """VlfmYoloParams (include/vlfm_b200.h)"""
+    _fields_ = [("conf_thres", C.c_float), ("iou_thres", C.c_float), ("agnostic", C.c_int32), ("pad", C.c_int32),
+                ("class_mask", C.c_uint32 * 4)]
 
 
 _P = C.c_void_p
@@ -131,6 +138,16 @@ _SIGNATURES = {
     "vlfm_pointnav_lstm_prep": (C.c_int, [_P, _P, _P, C.c_int] + [_P] * 9 + [C.c_int, _P]),
     "vlfm_pointnav_lstm_cell": (C.c_int, [_P, _P, _P, C.c_int, _P]),
     "vlfm_pointnav_lstm_head": (C.c_int, [_P] * 5 + [C.c_int] + [_P] * 6 + [C.c_int, _P]),
+    "vlfm_yolo_preprocess": (C.c_int, [_P, _P] + [C.c_int] * 5 + [_P] * 7),
+    "vlfm_yolo_im2col3x3": (C.c_int, [_P, C.c_int, _P] + [C.c_int] * 6 + [_P]),
+    "vlfm_yolo_maxpool2": (C.c_int, [_P, C.c_int, _P] + [C.c_int] * 5 + [_P]),
+    "vlfm_yolo_spp_pools": (C.c_int, [_P, C.c_int, _P] + [C.c_int] * 5 + [_P]),
+    "vlfm_yolo_upsample2": (C.c_int, [_P, C.c_int, _P] + [C.c_int] * 5 + [_P]),
+    "vlfm_yolo_add": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_longlong, C.c_int, _P]),
+    "vlfm_yolo_decode": (C.c_int, [_P] + [C.c_int] * 6 + [_P, C.c_float, C.c_int, C.c_int, _P, _P, _P, _P]),
+    "vlfm_yolo_sort": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
+    "vlfm_yolo_nms": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P]),
+    "vlfm_yolo_boxes": (C.c_int, [_P, _P, _P] + [C.c_int] * 3 + [C.c_float] * 3 + [C.c_int] * 2 + [_P] * 5),
 }
 
 _lib = None

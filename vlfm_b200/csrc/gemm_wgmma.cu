@@ -140,6 +140,8 @@ static_assert(SK_SLAB_ROWS == BM + GEMM_TAIL_MAX && SK_TILE == BM, "stream-K sla
 constexpr int GEMM_TAIL_KMAX = 6144;   // K elements of one CTA's slice that fit the tail-row staging buffer
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
+// torch's SiLU in fp32 (the opmath of its fp16 kernel)
+__device__ __forceinline__ float silu(float x) { return x / (1.f + expf(-x)); }
 
 // One column pair (n, n + 1) of one output row: activation, conversion and the store the epilogue kind asks for.
 // v0 / v1 already carry the bias.  `pair` = column n + 1 exists.
@@ -173,9 +175,17 @@ __device__ __forceinline__ void epilogue_store2(const GemmArgs& g, int row, int 
   }
 }
 
+// VLFM_EPI_BIAS_SILU_F16: SiLU -> fp16.  Its own kernel instantiation (SILU = true below), so that the other epilogues' code is
+// exactly what it was without it.
+__device__ __forceinline__ void epilogue_store2_silu(const GemmArgs& g, int row, int n, float v0, float v1, bool pair) {
+  __half* o = reinterpret_cast<__half*>(g.out) + (size_t)row * g.ldo + n;
+  const __half2 h = __floats2half2_rn(silu(v0), silu(v1));
+  if (pair) *reinterpret_cast<__half2*>(o) = h; else o[0] = __low2half(h);
+}
+
 // Epilogue of one warp's 16 x BN accumulator slab, straight from the wgmma fragment.  `row0` = first row of the slab;
 // `sbias` = this tile's bias slice in shared memory (zero-filled past N / without bias), added when `addb` (the first K split).
-template <int BN>
+template <int BN, bool SILU = false>
 __device__ __forceinline__ void epilogue_frag(const float (&acc)[BN / 2], int row0, int n_blk, const GemmArgs& g, bool split, bool addb, const float* sbias) {
   const int lane = threadIdx.x & 31;
   const int r_up = row0 + (lane >> 2), cq = (lane & 3) * 2;
@@ -185,8 +195,13 @@ __device__ __forceinline__ void epilogue_frag(const float (&acc)[BN / 2], int ro
     if (n >= g.N) continue;
     const bool pair = n + 1 < g.N;
     const float b0 = addb ? sbias[cl] : 0.f, b1 = addb ? sbias[cl + 1] : 0.f;
-    if (r_up < g.M) epilogue_store2(g, r_up, n, acc[4 * j] + b0, acc[4 * j + 1] + b1, pair, split);
-    if (r_up + 8 < g.M) epilogue_store2(g, r_up + 8, n, acc[4 * j + 2] + b0, acc[4 * j + 3] + b1, pair, split);
+    if constexpr (SILU) {
+      if (r_up < g.M) epilogue_store2_silu(g, r_up, n, acc[4 * j] + b0, acc[4 * j + 1] + b1, pair);
+      if (r_up + 8 < g.M) epilogue_store2_silu(g, r_up + 8, n, acc[4 * j + 2] + b0, acc[4 * j + 3] + b1, pair);
+    } else {
+      if (r_up < g.M) epilogue_store2(g, r_up, n, acc[4 * j] + b0, acc[4 * j + 1] + b1, pair, split);
+      if (r_up + 8 < g.M) epilogue_store2(g, r_up + 8, n, acc[4 * j + 2] + b0, acc[4 * j + 3] + b1, pair, split);
+    }
   }
 }
 
@@ -215,7 +230,7 @@ __device__ __forceinline__ void segment_store_frag(const float (&acc)[BN / 2], i
 // (blockIdx.x, blockIdx.y) and the K-blocks of split blockIdx.z.  A stream-K launch (g.sk.ctas > 0, 1-D grid) gives it a range
 // of the sequence of all tiles' K-blocks (SplitK in common.cuh), which may cover parts of two tiles: the producer streams straight
 // across the tile boundary, and the consumers finish a segment there (store it to the workspace, zero the accumulators) and go on.
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool SILU = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmArgs g) {
   constexpr uint32_t A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2;
@@ -403,8 +418,9 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 }
                 float v = tacc[r] + (addb ? sbias[f] : 0.f);
                 const size_t o = (size_t)(g.tail_row0 + r) * g.ldo + n;
-                if (g.epi == VLFM_EPI_BIAS_F16 || g.epi == VLFM_EPI_BIAS_GELU_F16 || g.epi == VLFM_EPI_BIAS_RELU_F16) {
-                  if (g.epi == VLFM_EPI_BIAS_GELU_F16) v = gelu_erf(v);
+                if (SILU || g.epi == VLFM_EPI_BIAS_F16 || g.epi == VLFM_EPI_BIAS_GELU_F16 || g.epi == VLFM_EPI_BIAS_RELU_F16) {
+                  if constexpr (SILU) v = silu(v);
+                  else if (g.epi == VLFM_EPI_BIAS_GELU_F16) v = gelu_erf(v);
                   else if (g.epi == VLFM_EPI_BIAS_RELU_F16) v = fmaxf(v, 0.f);
                   reinterpret_cast<__half*>(g.out)[o] = __float2half_rn(v);
                 } else {
@@ -420,7 +436,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         if (sk) {
           segment_store_frag<BN>(acc, wg * 64 + wq * 16, n_blk, g, addb, slab);
         } else {
-          epilogue_frag<BN>(acc, m_blk * BM + wg * 64 + wq * 16, n_blk, g, split, addb, sbias);
+          epilogue_frag<BN, SILU>(acc, m_blk * BM + wg * 64 + wq * 16, n_blk, g, split, addb, sbias);
         }
       }
       if (++s == STAGES) { s = 0; ph ^= 1; }
@@ -776,8 +792,11 @@ static int make_map(CUtensorMap* m, const void* base, int rows, int cols, int ld
   return VLFM_OK;
 }
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool SILU = false>
 static int launch_gemm(const CUtensorMap& ta, const void* W, int ldw, const GemmArgs& g, cudaStream_t st) {
+  if constexpr (!SILU) {
+    if (g.epi == VLFM_EPI_BIAS_SILU_F16) return launch_gemm<BN, STAGES, true>(ta, W, ldw, g, st);
+  }
   CUtensorMap tb;
   int rc = make_map(&tb, W, g.N, g.K, ldw, BN);
   if (rc) return rc;
@@ -786,14 +805,14 @@ static int launch_gemm(const CUtensorMap& ta, const void* W, int ldw, const Gemm
   static_assert(smem <= 227 * 1024, "GEMM stage ring exceeds the 227 KB a block may use");
   static bool configured = false;
   if (!configured) {
-    rc = check_cuda(cudaFuncSetAttribute(gemm_f16_wgmma_kernel<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute(gemm)");
+    rc = check_cuda(cudaFuncSetAttribute(gemm_f16_wgmma_kernel<BN, STAGES, SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute(gemm)");
     if (rc) return rc;
     configured = true;
   }
   const int num_k = (g.K + BK - 1) / BK;
   dim3 grid((g.N + BN - 1) / BN, g.tail_rows > 0 ? g.M / BM : (g.M + BM - 1) / BM, (num_k + g.kb_per_split - 1) / g.kb_per_split);
   if (g.sk.ctas > 0) grid = dim3(g.sk.ctas);
-  rc = check_cuda(launch_pdl(gemm_f16_wgmma_kernel<BN, STAGES>, grid, dim3(GEMM_THREADS), smem, st, ta, tb, g), "gemm_f16_wgmma_kernel");
+  rc = check_cuda(launch_pdl(gemm_f16_wgmma_kernel<BN, STAGES, SILU>, grid, dim3(GEMM_THREADS), smem, st, ta, tb, g), "gemm_f16_wgmma_kernel");
   if (rc) return rc;
   count_launch();
   return VLFM_OK;
@@ -891,9 +910,10 @@ extern "C" int vlfm_gemm_f16(const void* d_A, const void* d_W, const float* d_bi
   if (!d_A || !d_W || !d_out || M < 1 || N < 1 || K < 1) { set_error("vlfm_gemm_f16: bad argument"); return VLFM_E_INVALID; }
   if ((K & 7) || (lda & 7) || (ldw & 7) || (ldo & 7) || ((uintptr_t)d_A & 15) || ((uintptr_t)d_W & 15) || ((uintptr_t)d_out & 15)) {
     set_error("vlfm_gemm_f16: K, lda, ldw, ldo must be multiples of 8 and pointers 16-byte aligned"); return VLFM_E_INVALID; }
-  const bool csplit = (epilogue & VLFM_EPI_CLUSTER_SPLIT) != 0;
+  // the cluster-split kernel has no SiLU instantiation: that epilogue ignores the flag
+  const bool csplit = (epilogue & VLFM_EPI_CLUSTER_SPLIT) != 0 && (epilogue & ~VLFM_EPI_CLUSTER_SPLIT) != VLFM_EPI_BIAS_SILU_F16;
   epilogue &= ~VLFM_EPI_CLUSTER_SPLIT;
-  if (epilogue < 0 || epilogue > 4) { set_error("vlfm_gemm_f16: unknown epilogue %d", epilogue); return VLFM_E_INVALID; }
+  if (epilogue < 0 || (epilogue > 4 && epilogue != VLFM_EPI_BIAS_SILU_F16)) { set_error("vlfm_gemm_f16: unknown epilogue %d", epilogue); return VLFM_E_INVALID; }
   GemmArgs g{d_bias, d_out, M, N, K, ldo, epilogue, (K + BK - 1) / BK, 0, nullptr, 0, 0, 0, nullptr, BM};
   return gemm_dispatch(d_A, d_W, M, N, K, lda, ldw, g, stream, nullptr, 0, nullptr, csplit);
 }

@@ -147,14 +147,22 @@ def _placeholder(module: str, name: str) -> type:
 class RestrictedUnpickler(pickle.Unpickler):
     """Rebuilds tensors, builtins, ``collections.OrderedDict`` / ``defaultdict``, ``typing`` names and ``operator.getitem``;
     classes under omegaconf / habitat / habitat_baselines / vlfm become inert placeholders; any other global raises
-    ``pickle.UnpicklingError`` before it is called."""
+    ``pickle.UnpicklingError`` before it is called.  Subclasses (vlm/yolov7_weights.py) add placeholders through ``placeholder``
+    and name their file kind in ``what``."""
+
+    what = "PointNav checkpoint"
+
+    def placeholder(self, module, name):
+        """The stand-in class for global ``module.name``, or None when it gets none."""
+        return _placeholder(module, name) if module.split(".")[0] in _PLACEHOLDER_ROOTS else None
 
     def find_class(self, module, name):
-        if module.split(".")[0] in _PLACEHOLDER_ROOTS:
-            return _placeholder(module, name)
+        cls = self.placeholder(module, name)
+        if cls is not None:
+            return cls
         if name in _ALLOWED.get(module, ()):
             return super().find_class(module, name)
-        raise pickle.UnpicklingError(f"PointNav checkpoint: refusing to load global {module}.{name}")
+        raise pickle.UnpicklingError(f"{self.what}: refusing to load global {module}.{name}")
 
 
 def _restricted_load(f, **kwargs):
