@@ -233,6 +233,13 @@ int vlfm_attention_f32(const float* d_q, const float* d_k, const float* d_v, voi
  * VLFM_E_INVALID for NULL pointers, B < 1, P < 1 or ldo < P. */
 int vlfm_itc_head(const float* d_proj, const float* d_text, float* d_out, int B, int Q, int D, void* stream);
 int vlfm_itc_head_multi(const float* d_proj, const float* d_text, float* d_out, int B, int P, int Q, int D, int ldo, void* stream);
+/* im2col of a k x k conv (k = 1 or 3, zero padding k/2, stride 1 or 2) for vlfm_gemm_f16, shared by every conv net here (MobileSAM,
+ * PointNav, YOLOv7, the GroundingDINO neck).  d_x16 [B,H,W,C] fp16 with row stride ldx (elements; a channel slice of a wider
+ * buffer is fine) -> d_col16 [B*Ho*Wo, ldk] fp16, Ho = (H-1)/stride + 1 (Wo likewise), column (ky*k + kx)*C + c, columns >= k*k*C
+ * zero.  The conv weight is [O, ldk] in the same column order (vlm/dense.py::conv_rows).  ldx >= C; ldk >= k*k*C, ldk % 8 == 0;
+ * d_col16 16-byte aligned.  Any C, ldx and input alignment; C, ldx multiples of 8 with d_x16 16-byte aligned read 16 bytes at a
+ * time.  VLFM_E_INVALID otherwise, and for NULL pointers or B, H, W, C < 1. */
+int vlfm_im2col_f16(const void* d_x16, int ldx, void* d_col16, int B, int H, int W, int C, int k, int stride, int ldk, void* stream);
 
 /* ----------------------------------------------- GroundingDINO Swin-T backbone ---- */
 /* Replaces the image branch of groundingdino's predict() up to the backbone feature maps
@@ -287,7 +294,6 @@ int vlfm_cast_addpos_f16(const float* d_x, const float* d_pos, void* d_out_x16, 
  * backbone and the (boxes, logits) pair and outside the encoder / decoder layers (vlm/gdino_forward.py; module graph:
  * HF GroundingDinoModel.forward / GroundingDinoForObjectDetection.forward).
  * groupnorm_rows: torch.nn.GroupNorm of the neck on NHWC rows y [B,HW,C] -> d_out[b, row_off + i, :] of a [B,S,C] buffer.
- * im2col3x3s2: rows [B,h,w,C] fp32 -> fp16 [B*ho*wo, 9*C] ((ky,kx,c) order) for the fourth level's 3x3 stride-2 conv.
  * mask_rows_f16: fp32 rows -> fp16 GEMM operand with invalid rows zeroed (generate_encoder_output_proposals).
  * proposal_scores: score[b,s] = max_t <q[b,s,:], text[b,t,:]> (encoder_output_class_embed + max(-1)).
  * topk_rows: indices of the k best scores per image, descending, ties to the lower index (torch.topk; one-block bitonic sort for S <= 16384, radix select + sort of the k winners above, k <= 16384).
@@ -295,7 +301,6 @@ int vlfm_cast_addpos_f16(const float* d_x, const float* d_pos, void* d_out_x16, 
  * box_finish: sigmoid(delta + logit(ref, eps=1e-5)).   contrastive_sigmoid: sigmoid(<hs, text>) padded with 0 to L.       */
 int vlfm_groupnorm_rows(const float* d_y, int B, int HW, int C, int groups, const float* d_gamma, const float* d_beta, float eps,
                         float* d_out, int row_off, int S, void* stream);
-int vlfm_im2col3x3s2(const float* d_x, void* d_col16, int B, int h, int w, int C, void* stream);
 int vlfm_mask_rows_f16(const float* d_x, const uint8_t* d_valid, void* d_out16, long rows, int D, void* stream);
 int vlfm_proposal_scores(const float* d_q, const float* d_text, int B, int S, int T, int D, float* d_scores, void* stream);
 int vlfm_topk_rows(const float* d_scores, int B, int S, int k, long long* d_idx, void* stream);
@@ -408,15 +413,14 @@ int vlfm_render_draw(int G, int batch, uint8_t* d_frames, const int32_t* h_lists
 
 /* ------------------------------------------------------------------ MobileSAM ---- */
 /* Replaces MobileSAM.segment_bbox (vlfm/vlm/sam.py:40-57: SamPredictor.set_image + predict(box, multimask_output=False)) with the
- * TinyViT-5M encoder and the box-prompted mask decoder (engine: vlfm_b200/vlm/sam_engine.py).  GEMMs, LayerNorms and the 7-key
- * attentions run on vlfm_gemm_f16 / vlfm_gemm_f16_resid_ln / vlfm_layernorm / vlfm_attention_f16; these are the rest.
+ * TinyViT-5M encoder and the box-prompted mask decoder (engine: vlfm_b200/vlm/sam_engine.py).  GEMMs, LayerNorms, the 7-key
+ * attentions and the 3x3 convs' rows run on vlfm_gemm_f16 / vlfm_gemm_f16_resid_ln / vlfm_layernorm / vlfm_attention_f16 /
+ * vlfm_im2col_f16; these are the rest.
  *
  * vlfm_sam_preprocess: ResizeLongestSide(S): Pillow-exact bilinear resize [B,H,W,3] uint8 -> (OH, OW) (tables as for
  *   vlfm_preprocess_im2col, built by vlm/preprocess.py::bilinear_tables), horizontal pass first into d_mid [B,H,OW,3] uint8
  *   scratch, or with v_first = 1 (Pillow's order for frames more than 100x taller than wide that shrink vertically, see
  *   vlm/preprocess.py::pillow_vertical_first) vertical first into d_mid [B,OH,W,3]; then (x - mean) / std in fp32 (h_mean3 / h_std3: HOST float[3] on the 0..255 scale) and a zero pad to S x S -> d_out [B,S,S,3] fp16.
- * vlfm_sam_im2col3x3: fp16 NHWC [B,H,W,C] -> fp16 [B*Ho*Wo, ldk] rows of a 3x3 conv (pad 1, stride 1 or 2), column (ky*3+kx)*C + c,
- *   columns >= 9*C zero.  ldk % 8 == 0.
  * vlfm_sam_dwconv3x3: depthwise 3x3 conv (pad 1, stride 1 or 2), NHWC, weights d_w [9, C] (tap-major, BatchNorm folded) + d_b [C],
  *   then GELU when gelu != 0.  Input and output are fp32 (flag 1) or fp16 (0).
  * vlfm_sam_add_act: out = act(a + b) over n elements (b may be NULL; act = GELU when gelu != 0) -> d_out32 and / or d_out16.
@@ -440,7 +444,6 @@ int vlfm_render_draw(int G, int batch, uint8_t* d_frames, const int32_t* h_lists
 int vlfm_sam_preprocess(const uint8_t* d_img, uint8_t* d_mid, void* d_out, int B, int H, int W, int OH, int OW, int S,
                         const int32_t* d_hbounds, const int32_t* d_hkk, int hksize, const int32_t* d_vbounds, const int32_t* d_vkk,
                         int vksize, int v_first, const float* h_mean3, const float* h_std3, void* stream);
-int vlfm_sam_im2col3x3(const void* d_x16, void* d_col16, int B, int H, int W, int C, int stride, int ldk, void* stream);
 int vlfm_sam_dwconv3x3(const void* d_in, int in_f32, const float* d_w, const float* d_b, void* d_out, int out_f32, int B, int H, int W,
                        int C, int stride, int gelu, void* stream);
 int vlfm_sam_add_act(const float* d_a, const float* d_b, float* d_out32, void* d_out16, long long n, int gelu, void* stream);
@@ -461,7 +464,7 @@ int vlfm_sam_mask_finish(const float* d_low, uint8_t* d_out, int M, int L, int S
 /* ------------------------------------------------------------------ PointNav ---- */
 /* Replaces WrappedPointNavResNetPolicy.act (vlfm/policy/utils/pointnav_policy.py:51-128): the ResNet-18 depth encoder with
  * GroupNorm and the 2-layer LSTM of 512 (engine: vlfm_b200/policy/pointnav_engine.py).  Activations are NHWC.  Each conv is an
- * im2col pass (vlfm_pointnav_depth_in, vlfm_sam_im2col3x3, vlfm_pointnav_gather_s2) plus vlfm_gemm_f16 with VLFM_EPI_BIAS_F32;
+ * im2col pass (vlfm_pointnav_depth_in for conv1, vlfm_im2col_f16 for the others) plus vlfm_gemm_f16 with VLFM_EPI_BIAS_F32;
  * these are the rest.  Every reduction has a fixed order: bitwise reproducible, and independent of the other environments.
  *
  * vlfm_pointnav_depth_in: d_depth [B,H,W] fp32 -> torch "area" resize to (IH, IW) (adaptive average pooling, fp32) -> 2x2
@@ -472,7 +475,6 @@ int vlfm_sam_mask_finish(const float* d_low, uint8_t* d_out, int M, int L, int S
  *   square root), then out = act(GN_a(x) + r) -> d_out32 (may alias d_r) and / or d_out16.  rmode 0: r = 0; 1: r = d_r (fp32
  *   [B,HW,C]); 2: r = GN_b(d_y) (the downsample branch, its own statistics).  act = ReLU when relu != 0.
  * vlfm_pointnav_maxpool3s2: 3x3 stride-2 pad-1 max pool (padding is -inf) of d_x [B,H,W,C] fp32 -> d_out32 and / or d_out16.
- * vlfm_pointnav_gather_s2: the rows of a 1x1 stride-2 conv: d_out16 [B*Ho*Wo, C] = d_x16 [B, 2yo, 2xo, :] fp16, C % 8 == 0.
  * vlfm_pointnav_gemv_f32: d_y[b*ldy + n] = act(sum_k d_x[b*ldx + k] d_W[n*ldw + k] + d_bias[n]) in fp32 on CUDA cores, B <= 64;
  *   W is read once for all B.  Each (b, n) is summed in an order that depends on K only (bitwise the same for any B).
  *   K, ldx, ldw multiples of 4; d_x, d_W 16-byte aligned; d_bias may be NULL.
@@ -493,7 +495,6 @@ int vlfm_pointnav_groupnorm(const float* d_x, const float* d_gamma_a, const floa
                             const float* d_y, const float* d_gamma_b, const float* d_beta_b, float* d_out32, void* d_out16, int B, int HW,
                             int C, int G, float eps, int relu, void* stream);
 int vlfm_pointnav_maxpool3s2(const float* d_x, float* d_out32, void* d_out16, int B, int H, int W, int C, void* stream);
-int vlfm_pointnav_gather_s2(const void* d_x16, void* d_out16, int B, int H, int W, int C, void* stream);
 int vlfm_pointnav_gemv_f32(const float* d_x, int ldx, const float* d_W, int ldw, const float* d_bias, float* d_y, int ldy, int B, int N,
                            int K, int relu, void* stream);
 int vlfm_pointnav_lstm_prep(const int32_t* d_env_ids, const float* d_state, const void* d_prev, int discrete, const uint8_t* d_masks,
@@ -507,15 +508,13 @@ int vlfm_pointnav_lstm_head(const float* d_gates, const float* d_cbuf, const flo
 /* ------------------------------------------------------------------ YOLOv7 ---- */
 /* Replaces YOLOv7.predict (vlfm/vlm/yolov7.py:50-110): YOLOv7-E6E in fp16 plus yolov7's non_max_suppression and scale_coords
  * (engine: vlfm_b200/vlm/yolov7_engine.py).  Activations are fp16 NHWC rows with a row stride ld* (elements), so a layer may read
- * or write one channel slice of a concat buffer.  1x1 convs are vlfm_gemm_f16 on the rows, 3x3 convs vlfm_yolo_im2col3x3 plus
+ * or write one channel slice of a concat buffer.  1x1 convs are vlfm_gemm_f16 on the rows, 3x3 convs vlfm_im2col_f16 plus
  * vlfm_gemm_f16, both with VLFM_EPI_BIAS_SILU_F16; these are the rest.  Results are bitwise reproducible.
  *
  * vlfm_yolo_preprocess: cv2.resize(INTER_AREA) of d_img [B,H,W,3] uint8 to (OH, OW) (H >= OH, W >= OW; cv2's area tables in CSR
  *   form, built on the host by vlm/yolov7_engine.py: per destination row dy the entries d_yofs[dy]..d_yofs[dy+1] of (d_ysi, d_ybeta),
  *   per destination column likewise), fp16(v / 255), then ReOrg: d_out16 [B, OH/2, OW/2, 16], channel g*3 + c with g = (y & 1) +
  *   2 * (x & 1), channels 12..15 zero.
- * vlfm_yolo_im2col3x3: d_x16 [B,H,W,C] (row stride ldx) -> d_col16 [B*Ho*Wo, ldk] rows of a 3x3 conv, pad 1, stride 1 or 2, column
- *   (ky*3+kx)*C + c, columns >= 9C zero.  C, ldx, ldk multiples of 8.
  * vlfm_yolo_maxpool2: MaxPool2d(2, 2) [B,H,W,C] (ldx) -> [B,H/2,W/2,C] (ldo).
  * vlfm_yolo_spp_pools: MaxPool2d(k, 1, k/2) for k = 5, 9, 13 of [B,H,W,C] (ldx) -> d_out16 + j*C (ldo) for the j-th.
  * vlfm_yolo_upsample2: nearest x2 [B,H,W,C] (ldx) -> [B,2H,2W,C] (ldo); C, ldx, ldo multiples of 8.
@@ -537,7 +536,6 @@ typedef struct VlfmYoloParams {
 int vlfm_yolo_preprocess(const uint8_t* d_img, void* d_out16, int B, int H, int W, int OH, int OW, const int32_t* d_yofs,
                          const int32_t* d_ysi, const float* d_ybeta, const int32_t* d_xofs, const int32_t* d_xsi, const float* d_xalpha,
                          void* stream);
-int vlfm_yolo_im2col3x3(const void* d_x16, int ldx, void* d_col16, int B, int H, int W, int C, int stride, int ldk, void* stream);
 int vlfm_yolo_maxpool2(const void* d_x16, int ldx, void* d_out16, int ldo, int B, int H, int W, int C, void* stream);
 int vlfm_yolo_spp_pools(const void* d_x16, int ldx, void* d_out16, int ldo, int B, int H, int W, int C, void* stream);
 int vlfm_yolo_upsample2(const void* d_x16, int ldx, void* d_out16, int ldo, int B, int H, int W, int C, void* stream);

@@ -1,5 +1,5 @@
 """vlm/dense.py is the only Python code in the package that calls the dense C-ABI entry points (GEMMs, LayerNorms, attention,
-x2 split, casts): every engine goes through its wrappers instead of marshalling those ctypes calls itself."""
+x2 split, casts, conv im2col): every engine goes through its wrappers instead of marshalling those ctypes calls itself."""
 import ast
 import os
 
@@ -10,7 +10,7 @@ PACKAGE = os.path.join(ROOT, "vlfm_b200")
 DENSE = os.path.join(PACKAGE, "vlm", "dense.py")
 ENTRY_POINTS = {
     "vlfm_gemm_f16", "vlfm_gemm_f16_resid_ln", "vlfm_gemm_f16x2", "vlfm_gemm_f16x2_resid_ln", "vlfm_layernorm", "vlfm_layernorm_x2",
-    "vlfm_attention_f16", "vlfm_attention_f32", "vlfm_split_x2", "vlfm_cast_f32_f16", "vlfm_cast_addpos_f16",
+    "vlfm_attention_f16", "vlfm_attention_f32", "vlfm_split_x2", "vlfm_cast_f32_f16", "vlfm_cast_addpos_f16", "vlfm_im2col_f16",
 }
 
 

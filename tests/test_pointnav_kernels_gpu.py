@@ -133,10 +133,10 @@ def test_groupnorm_in_place_residual():
     assert torch.equal(out, r2)
 
 
-# ------------------------------------------------------------------------------------------------------ pool and gather
+# ------------------------------------------------------------------------------------------------------------ max pool
 @pytest.mark.gpu
 @pytest.mark.parametrize("H,W,C", [(112, 112, 32), (106, 120, 32), (7, 9, 8), (1, 3, 16)])
-def test_maxpool_and_gather(H, W, C):
+def test_maxpool3s2(H, W, C):
     B = 2
     x = torch.randn(B, H, W, C)
     Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
@@ -146,11 +146,6 @@ def test_maxpool_and_gather(H, W, C):
     ref = F.max_pool2d(x.permute(0, 3, 1, 2), 3, 2, 1).permute(0, 2, 3, 1)
     assert torch.equal(o32.cpu(), ref)
     assert torch.equal(o16.cpu(), ref.half())
-    if C % 8 == 0:
-        x16 = dx.half()
-        g = _nan(B * Ho * Wo, C, dtype=torch.float16)
-        _call("vlfm_pointnav_gather_s2", x16.data_ptr(), g.data_ptr(), B, H, W, C, _st())
-        assert torch.equal(g.cpu(), x16.cpu()[:, ::2, ::2, :].reshape(-1, C))
 
 
 # ---------------------------------------------------------------------------------------------------------------- GEMV
@@ -273,7 +268,7 @@ def test_head_argmax_first_index_on_ties():
 
 # --------------------------------------------------------------------------------------------------------- bad arguments
 @pytest.mark.gpu
-def test_bad_arguments():
+def test_bad_arguments_are_refused():
     lib = _lib().load()
     p = torch.zeros(4096, device="cuda")
     a = p.data_ptr()
@@ -288,8 +283,6 @@ def test_bad_arguments():
         lambda: lib.vlfm_pointnav_groupnorm(a, a, a, 3, None, None, None, None, a, None, 1, 4, 32, 16, 1e-5, 1, st),
         lambda: lib.vlfm_pointnav_groupnorm(a, a, a, 0, None, None, None, None, None, None, 1, 4, 32, 16, 1e-5, 1, st),  # no output
         lambda: lib.vlfm_pointnav_maxpool3s2(a, None, None, 1, 4, 4, 8, st),
-        lambda: lib.vlfm_pointnav_gather_s2(a, a, 1, 4, 4, 12, st),                        # C % 8
-        lambda: lib.vlfm_pointnav_gather_s2(a + 2, a, 1, 4, 4, 16, st),                    # misaligned
         lambda: lib.vlfm_pointnav_gemv_f32(a, 8, a, 8, None, a, 8, 0, 8, 8, 0, st),
         lambda: lib.vlfm_pointnav_gemv_f32(a, 8, a, 8, None, a, 8, 65, 8, 8, 0, st),
         lambda: lib.vlfm_pointnav_gemv_f32(a, 8, a, 8, None, a, 8, 1, 8, 6, 0, st),        # K % 4
@@ -306,7 +299,7 @@ def test_bad_arguments():
     assert _lib().launch_count() == n0
 
 
-def test_pointnav_ptxas_no_spills(tmp_path):
+def test_pointnav_kernels_do_not_spill(tmp_path):
     if not shutil.which(build.NVCC) and not os.path.exists(build.NVCC):
         pytest.skip("nvcc not available")
     src = os.path.join(build.CSRC, "pointnav.cu")
@@ -316,6 +309,6 @@ def test_pointnav_ptxas_no_spills(tmp_path):
     log = r.stdout + r.stderr
     props = re.findall(r"Function properties for (\S+)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", log)
     kernels = [p for p in props if "pointnav" in p[0]]
-    assert len(kernels) >= 14        # 7 GEMV instantiations + 7 others
+    assert len(kernels) >= 13        # 7 GEMV instantiations + 6 others
     for name, _, st, ld in kernels:
         assert st == "0" and ld == "0", f"{name} spills ({st} B stores, {ld} B loads)"

@@ -406,37 +406,7 @@ def test_dwconv3x3_engine_shapes(H, W, C, stride, gelu, in_f32, out_f32):
     assert ok
 
 
-# ================================================================================================ 4. im2col ====
-def ref_im2col(x, stride, ldk):
-    """F.unfold (pad 1) reordered to columns (ky, kx, c), zero-padded to ldk"""
-    B, H, W, C = x.shape
-    u = F.unfold(x.float().permute(0, 3, 1, 2), 3, padding=1, stride=stride)          # [B, C*9, L], rows (c, ky, kx)
-    L = u.shape[-1]
-    r = u.view(B, C, 9, L).permute(0, 3, 2, 1).reshape(B * L, 9 * C)
-    return F.pad(r, (0, ldk - 9 * C)).half()
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("B,H,W,C,stride,ldk", [(2, 17, 23, 3, 2, 32), (1, 64, 64, 3, 2, 32), (2, 9, 11, 256, 1, 2304),
-                                                  (1, 16, 16, 256, 1, 2304), (2, 7, 5, 5, 1, 48), (2, 7, 5, 5, 2, 48),
-                                                  (1, 1, 1, 5, 2, 48), (3, 13, 8, 32, 2, 288)])
-def test_im2col3x3_is_the_unfold(B, H, W, C, stride, ldk):
-    x = torch.randn(B, H, W, C, generator=torch.Generator().manual_seed(H * W + C)).half()
-    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
-    n = B * Ho * Wo
-    xd = x.cuda()
-    outs = []
-    for _ in range(2):
-        col, sent = _out(n, ldk, torch.float16)
-        _call("vlfm_sam_im2col3x3", xd.data_ptr(), col.data_ptr(), B, H, W, C, stride, ldk, _lib().stream_ptr())
-        _check_written(col, sent, n, "im2col")
-        outs.append(col[:n].cpu())
-    ref = ref_im2col(x, stride, ldk)
-    assert torch.equal(_bits(outs[0]), _bits(ref)), f"{int((outs[0] != ref).sum())} of {ref.numel()} values differ"
-    assert torch.equal(_bits(outs[0]), _bits(outs[1]))
-
-
-# ============================================================================================= 5. box tokens ====
+# ============================================================================================= 4. box tokens ====
 def ref_box_tokens(boxes, hw, S, gauss, fixed, half_shift=True, scale=True, swap_xy=False, clamp=False):
     """apply_boxes in float64, cast to float32; then +0.5, /S, 2x - 1 and the Gaussian projection in float32 (HF's
     PositionEmbeddingRandom: a float32 matmul, so u*g0 and v*g1 rounded, then summed), 2 pi a in float32; sin / cos in float64
@@ -542,7 +512,7 @@ def test_box_tokens_match_reference(H, W, S, D):
         assert m > 10, f"the test cannot tell the kernel from a reference with {n}"
 
 
-# ============================================================================================ 6. mask finish ====
+# ============================================================================================ 5. mask finish ====
 def _lerp(o_size, in_size, align_corners=False):
     """torch upsample_bilinear2d's source indices and float32 weights for in_size -> o_size"""
     o = np.arange(o_size, dtype=np.float32)
@@ -660,7 +630,7 @@ def test_mask_finish_nan_low_gives_empty_mask():
     assert int(out[1].sum()) == 0 and bool((out <= 1).all()) and int(out[0].sum()) > 0
 
 
-# ============================================================================================ 7. mask logits ====
+# ============================================================================================ 6. mask logits ====
 def ref_mask_logits(up, hyper, M, h, w, C):
     """logits[m, Y, X] = sum_c hyper[m, c] GELU(up[m, Y/2, X/2, (Y%2, X%2), c]) in float64 -> (logits, bar)"""
     u = up.double().view(M, h, w, 2, 2, C).permute(0, 1, 3, 2, 4, 5).reshape(M, 2 * h, 2 * w, C)
@@ -694,7 +664,7 @@ def test_mask_logits_match_reference(M, h, w, C):
     assert bool((err <= bar).all())
 
 
-# ========================================================================================= 8. bit-exact ports ====
+# ========================================================================================= 7. bit-exact ports ====
 @pytest.mark.gpu
 @pytest.mark.parametrize("B,h,w,C", [(2, 3, 5, 7), (1, 64, 64, 64), (2, 16, 16, 32), (1, 1, 2, 1)])
 def test_pixel_shuffle2_scatter(B, h, w, C):
@@ -778,7 +748,7 @@ def test_add_act(n, with_b, gelu, inplace):
         assert torch.equal(_bits(o32[:n, 0]), _bits(ref))
 
 
-# ============================================================================================= 9. preprocess ====
+# ============================================================================================= 8. preprocess ====
 def _tables_dev(H, W, S):
     newh, neww = preshape(H, W, S)
     hb, hk, hks = bilinear_tables(W, neww)
@@ -856,9 +826,6 @@ def _bad_calls():
         ("vlfm_sam_preprocess", "v_first 2", pre(vf=2)),
         ("vlfm_sam_preprocess", "hksize 0", pre(hks=0)),
         ("vlfm_sam_preprocess", "NULL image", pre(img=None)),
-        ("vlfm_sam_im2col3x3", "ldk < 9C", (P, P, 1, 4, 4, 3, 1, 24, st)),
-        ("vlfm_sam_im2col3x3", "ldk % 8", (P, P, 1, 4, 4, 3, 1, 36, st)),
-        ("vlfm_sam_im2col3x3", "stride 3", (P, P, 1, 4, 4, 3, 3, 32, st)),
         ("vlfm_sam_dwconv3x3", "stride 0", (P, 0, Pf, Pf, P, 0, 1, 4, 4, 8, 0, 1, st)),
         ("vlfm_sam_dwconv3x3", "C 0", (P, 0, Pf, Pf, P, 0, 1, 4, 4, 0, 1, 1, st)),
         ("vlfm_sam_dwconv3x3", "NULL bias", (P, 0, Pf, None, P, 0, 1, 4, 4, 8, 1, 1, st)),
@@ -886,7 +853,7 @@ def _bad_calls():
 
 
 @pytest.mark.gpu
-def test_bad_arguments_are_refused_without_a_launch():
+def test_bad_arguments_launch_nothing():
     lib = _lib()
     L = lib.load()
     calls, bufs = _bad_calls()

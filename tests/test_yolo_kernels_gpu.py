@@ -94,19 +94,6 @@ def test_pools_upsample_add_bit_exact(lib):
     assert torch.equal(out, rows + y)
 
 
-@pytest.mark.parametrize("stride", [1, 2])
-def test_im2col_strided(lib, stride):
-    B, H, W, C, ld = 2, 9, 12, 24, 40
-    x = torch.randn(B, H, W, ld, device=dev).half()
-    xs = x[..., 8:8 + C]
-    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
-    col = nan16(B * Ho * Wo, 9 * C)
-    _lib.check(lib.vlfm_yolo_im2col3x3(xs.data_ptr(), ld, col.data_ptr(), B, H, W, C, stride, 9 * C, st()), "im2col")
-    ref = torch.nn.functional.unfold(xs.permute(0, 3, 1, 2).float(), 3, padding=1, stride=stride)   # [B, C*9, L] (c, ky, kx)
-    ref = ref.view(B, C, 9, -1).permute(0, 3, 2, 1).reshape(B * Ho * Wo, 9 * C).half()
-    assert torch.equal(col, ref)
-
-
 def decode_ref(head, nc, anchors, stride, conf):
     """float64 decode of one level [B, ny, nx, na*no] -> per frame {row: (x1, y1, x2, y2, conf, cls)}"""
     B, ny, nx, _ = head.shape
@@ -260,7 +247,7 @@ def test_boxes_against_float64(lib, hw):
         assert torch.all(boxes[b, k:] == 0) and torch.all(scores[b, k:] == 0) and torch.all(classes[b, k:] == -1)
 
 
-def test_bad_arguments(lib):
+def test_bad_arguments_are_refused(lib):
     x = torch.zeros(4096, dtype=F16, device=dev)
     f = torch.zeros(4096, device=dev)
     i = torch.zeros(4096, dtype=torch.int32, device=dev)
@@ -269,8 +256,6 @@ def test_bad_arguments(lib):
     cases = [
         lambda: lib.vlfm_yolo_preprocess(None, P, 1, 480, 640, 448, 640, i.data_ptr(), i.data_ptr(), f.data_ptr(), i.data_ptr(), i.data_ptr(), f.data_ptr(), None),
         lambda: lib.vlfm_yolo_preprocess(P, P, 1, 400, 640, 448, 640, i.data_ptr(), i.data_ptr(), f.data_ptr(), i.data_ptr(), i.data_ptr(), f.data_ptr(), None),
-        lambda: lib.vlfm_yolo_im2col3x3(P, 12, P, 1, 4, 4, 12, 1, 108, None),
-        lambda: lib.vlfm_yolo_im2col3x3(P, 16, P, 1, 4, 4, 16, 3, 144, None),
         lambda: lib.vlfm_yolo_maxpool2(P, 4, P, 8, 1, 4, 4, 8, None),
         lambda: lib.vlfm_yolo_spp_pools(P, 8, P, 16, 1, 4, 4, 8, None),
         lambda: lib.vlfm_yolo_upsample2(P, 8, P, 8, 1, 4, 4, 4, None),

@@ -100,8 +100,8 @@ _SIGNATURES = {
     "vlfm_fill_small_holes_batch": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_double, _P, _P, C.c_size_t, _P, _P, C.c_size_t, _P]),
     "vlfm_itc_head": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "vlfm_itc_head_multi": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "vlfm_im2col_f16": (C.c_int, [_P, C.c_int, _P] + [C.c_int] * 7 + [_P]),
     "vlfm_groupnorm_rows": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_float, _P, C.c_int, C.c_int, _P]),
-    "vlfm_im2col3x3s2": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "vlfm_mask_rows_f16": (C.c_int, [_P, _P, _P, C.c_long, C.c_int, _P]),
     "vlfm_proposal_scores": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "vlfm_topk_rows": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, _P]),
@@ -119,7 +119,6 @@ _SIGNATURES = {
     "vlfm_render_draw": (C.c_int, [C.c_int, C.c_int, _P, _P, C.c_size_t, _P, C.c_size_t, _P]),
     "vlfm_sam_preprocess": (C.c_int, [_P, _P, _P] + [C.c_int] * 6 + [_P, _P, C.c_int, _P, _P, C.c_int, C.c_int,
                                       C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
-    "vlfm_sam_im2col3x3": (C.c_int, [_P, _P] + [C.c_int] * 6 + [_P]),
     "vlfm_sam_dwconv3x3": (C.c_int, [_P, C.c_int, _P, _P, _P] + [C.c_int] * 7 + [_P]),
     "vlfm_sam_add_act": (C.c_int, [_P, _P, _P, _P, C.c_longlong, C.c_int, _P]),
     "vlfm_sam_window_attention": (C.c_int, [_P, _P, _P, _P] + [C.c_int] * 6 + [C.c_float, _P]),
@@ -133,13 +132,11 @@ _SIGNATURES = {
     "vlfm_pointnav_depth_in": (C.c_int, [_P] + [C.c_int] * 5 + [_P, C.c_int, _P, _P]),
     "vlfm_pointnav_groupnorm": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, _P, _P] + [C.c_int] * 4 + [C.c_float, C.c_int, _P]),
     "vlfm_pointnav_maxpool3s2": (C.c_int, [_P, _P, _P] + [C.c_int] * 4 + [_P]),
-    "vlfm_pointnav_gather_s2": (C.c_int, [_P, _P] + [C.c_int] * 4 + [_P]),
     "vlfm_pointnav_gemv_f32": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P] + [C.c_int] * 5 + [_P]),
     "vlfm_pointnav_lstm_prep": (C.c_int, [_P, _P, _P, C.c_int] + [_P] * 9 + [C.c_int, _P]),
     "vlfm_pointnav_lstm_cell": (C.c_int, [_P, _P, _P, C.c_int, _P]),
     "vlfm_pointnav_lstm_head": (C.c_int, [_P] * 5 + [C.c_int] + [_P] * 6 + [C.c_int, _P]),
     "vlfm_yolo_preprocess": (C.c_int, [_P, _P] + [C.c_int] * 5 + [_P] * 7),
-    "vlfm_yolo_im2col3x3": (C.c_int, [_P, C.c_int, _P] + [C.c_int] * 6 + [_P]),
     "vlfm_yolo_maxpool2": (C.c_int, [_P, C.c_int, _P] + [C.c_int] * 5 + [_P]),
     "vlfm_yolo_spp_pools": (C.c_int, [_P, C.c_int, _P] + [C.c_int] * 5 + [_P]),
     "vlfm_yolo_upsample2": (C.c_int, [_P, C.c_int, _P] + [C.c_int] * 5 + [_P]),

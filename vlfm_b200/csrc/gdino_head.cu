@@ -1,6 +1,6 @@
 // GroundingDINO model-level kernels that are not inside an encoder / decoder layer (vlfm_b200/vlm/gdino_forward.py):
-// neck GroupNorm on NHWC rows, im2col of the fourth level's 3x3 stride-2 convolution, two-stage proposal scoring,
-// language-guided top-k query selection, row gather, box / class heads.
+// neck GroupNorm on NHWC rows (the fourth level's 3x3 stride-2 conv is vlfm_im2col_f16 plus the GEMM), two-stage proposal
+// scoring, language-guided top-k query selection, row gather, box / class heads.
 //
 // Reference: groundingdino ... `model(image, captions=[caption])` called from vlfm/vlm/grounding_dino.py:61-67; the restated
 // module graph is HF `GroundingDinoModel.forward` (input_proj_vision, generate_encoder_output_proposals, encoder_output_class_embed,
@@ -45,26 +45,6 @@ groupnorm_rows_kernel(const float* __restrict__ y, int HW, int C, int groups, co
   for (int i = tid; i < n; i += 256) {
     const int r = i / cpg, c = i - r * cpg;
     ob[(size_t)r * C + c] = (base[(size_t)r * C + c] - mean) * rstd * gamma[g * cpg + c] + beta[g * cpg + c];
-  }
-}
-
-// ------------------------------------------------------------------------------------------ im2col ----
-// x [B, h, w, C] fp32 rows -> col [B*ho*wo, 9*C] fp16, column order (ky, kx, c); 3x3 kernel, stride 2, zero padding 1
-__global__ void im2col3x3s2_kernel(const float* __restrict__ x, __half* __restrict__ col, int B, int h, int w, int C, int ho, int wo) {
-  const long total = (long)B * ho * wo * 9 * (C / 4);
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const int c4 = (int)(i % (C / 4));
-    long r = i / (C / 4);
-    const int k = (int)(r % 9); r /= 9;
-    const int ox = (int)(r % wo); r /= wo;
-    const int oy = (int)(r % ho);
-    const int b = (int)(r / ho);
-    const int iy = 2 * oy - 1 + k / 3, ix = 2 * ox - 1 + k % 3;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if ((unsigned)iy < (unsigned)h && (unsigned)ix < (unsigned)w) v = *reinterpret_cast<const float4*>(x + (((size_t)b * h + iy) * w + ix) * C + 4 * c4);
-    __half2 h0 = __floats2half2_rn(v.x, v.y), h1 = __floats2half2_rn(v.z, v.w);
-    *reinterpret_cast<uint2*>(col + ((((size_t)b * ho + oy) * wo + ox) * 9 + k) * C + 4 * c4) =
-        make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
   }
 }
 
@@ -284,15 +264,6 @@ extern "C" int vlfm_groupnorm_rows(const float* d_y, int B, int HW, int C, int g
     set_error("vlfm_groupnorm_rows: bad argument"); return VLFM_E_INVALID; }
   groupnorm_rows_kernel<<<dim3(groups, B), 256, 0, (cudaStream_t)stream>>>(d_y, HW, C, groups, d_gamma, d_beta, eps, d_out, row_off, S);
   VLFM_CHECK_LAUNCH("groupnorm_rows_kernel");
-  count_launch();
-  return VLFM_OK;
-}
-
-extern "C" int vlfm_im2col3x3s2(const float* d_x, void* d_col16, int B, int h, int w, int C, void* stream) {
-  if (!d_x || !d_col16 || B < 1 || h < 1 || w < 1 || C < 4 || (C & 3)) { set_error("vlfm_im2col3x3s2: bad argument (C %% 4)"); return VLFM_E_INVALID; }
-  const int ho = (h + 2 - 3) / 2 + 1, wo = (w + 2 - 3) / 2 + 1;
-  im2col3x3s2_kernel<<<nb((long)B * ho * wo * 9 * (C / 4)), 256, 0, (cudaStream_t)stream>>>(d_x, (__half*)d_col16, B, h, w, C, ho, wo);
-  VLFM_CHECK_LAUNCH("im2col3x3s2_kernel");
   count_launch();
   return VLFM_OK;
 }

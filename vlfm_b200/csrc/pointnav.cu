@@ -1,11 +1,11 @@
 // PointNav policy kernels (vlfm/policy/utils/pointnav_policy.py WrappedPointNavResNetPolicy.act: a ResNet-18 over depth and a
 // 2-layer LSTM of 512); the engine is vlfm_b200/policy/pointnav_engine.py.  Activations are NHWC.  Every conv runs as an im2col
-// pass plus vlfm_gemm_f16 (fp16 operands, fp32 out); these kernels are the rest:
+// pass (conv1's below, the others vlfm_im2col_f16) plus vlfm_gemm_f16 (fp16 operands, fp32 out); these kernels are the rest:
 //   - pointnav_depth_in: area resize of the depth frame to the network's input size, 2x2 average pool, and the conv1 (7x7, stride
 //     2, pad 3) im2col rows, in one launch;
 //   - pointnav_groupnorm: GroupNorm statistics per (image, group) and out = act(GN_a(x) + r), r = none, an fp32 identity stream
 //     or GN_b(y) of the downsample branch, to fp32 and / or fp16;
-//   - pointnav_maxpool3s2, pointnav_gather_s2: the stem's max pool and the rows of a stride-2 1x1 conv;
+//   - pointnav_maxpool3s2: the stem's max pool;
 //   - pointnav_gemv: y = act(x W^T + b) in fp32 on CUDA cores, W streamed once for up to 64 environments' inputs;
 //   - pointnav_lstm_prep / pointnav_lstm_cell / pointnav_lstm_head: mask, goal and previous-action features, the LSTM cell
 //     updates, the action head and the hidden-state write-back.
@@ -159,18 +159,6 @@ __global__ void pointnav_maxpool3s2_kernel(const float* __restrict__ x, float* _
       }
     if (out32) out32[i] = m;
     if (out16) out16[i] = __float2half_rn(m);
-  }
-}
-
-// 8 fp16 (16 bytes) per thread: C % 8 == 0.
-__global__ void pointnav_gather_s2_kernel(const uint4* __restrict__ x, uint4* __restrict__ out, int B, int H, int W, int C8, int Ho,
-                                          int Wo) {
-  const long long n = (long long)B * Ho * Wo * C8;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const int c = (int)(i % C8);
-    const long long r = i / C8;
-    const int xo = (int)(r % Wo), yo = (int)((r / Wo) % Ho), b = (int)(r / ((long long)Wo * Ho));
-    out[i] = x[(((size_t)b * H + 2 * yo) * W + 2 * xo) * C8 + c];
   }
 }
 
@@ -393,16 +381,6 @@ extern "C" int vlfm_pointnav_maxpool3s2(const float* d_x, float* d_out32, void* 
   pointnav_maxpool3s2_kernel<<<pn_grid((long long)B * Ho * Wo * C, 256), 256, 0, (cudaStream_t)stream>>>(d_x, d_out32, (__half*)d_out16,
                                                                                                           B, H, W, C, Ho, Wo);
   PN_LAUNCHED("pointnav_maxpool3s2_kernel");
-  return VLFM_OK;
-}
-
-extern "C" int vlfm_pointnav_gather_s2(const void* d_x16, void* d_out16, int B, int H, int W, int C, void* stream) {
-  if (!d_x16 || !d_out16 || B < 1 || H < 1 || W < 1 || C < 8 || (C & 7) || !pn_aligned16(d_x16) || !pn_aligned16(d_out16)) {
-    set_error("vlfm_pointnav_gather_s2: bad argument"); return VLFM_E_INVALID; }
-  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-  pointnav_gather_s2_kernel<<<pn_grid((long long)B * Ho * Wo * (C / 8), 256), 256, 0, (cudaStream_t)stream>>>(
-      (const uint4*)d_x16, (uint4*)d_out16, B, H, W, C / 8, Ho, Wo);
-  PN_LAUNCHED("pointnav_gather_s2_kernel");
   return VLFM_OK;
 }
 

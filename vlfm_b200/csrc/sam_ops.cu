@@ -1,10 +1,9 @@
 // Operators of MobileSAM (TinyViT-5M image encoder + box-prompted two-way mask decoder) that no shared kernel covers (sm_90a).
 // Reference call site: vlfm/vlm/sam.py:40-57 (SamPredictor.set_image + predict(box=..., multimask_output=False)).
-// GEMMs, LayerNorms and the short attentions run on the shared kernels (vlfm_gemm_f16*, vlfm_layernorm, vlfm_attention_f16);
-// the engine is vlm/sam_engine.py.
+// GEMMs, LayerNorms and the short attentions run on the shared kernels (vlfm_gemm_f16*, vlfm_layernorm, vlfm_attention_f16), the
+// 3x3 convs on vlfm_im2col_f16 plus the GEMM; the engine is vlm/sam_engine.py.
 //   - sam_resize_pass / sam_resize_norm: Pillow-exact separable bilinear resize (ResizeLongestSide(1024)) in Pillow's pass
 //     order, the fp32 pixel normalisation (true division) and the zero pad to S x S, written as fp16 NHWC;
-//   - sam_im2col3x3: fp16 NHWC -> rows of a 3x3 (stride 1 or 2, pad 1) conv GEMM, K zero-padded to ldk;
 //   - sam_dwconv3x3: depthwise 3x3 conv with folded BatchNorm and optional GELU (TinyViT MBConv / PatchMerging / local_conv);
 //   - sam_add_act: out = act(a + b) (MBConv "add shortcut, then GELU"; plain casts);
 //   - sam_window_attention: TinyViT window attention (49- or 196-token windows, head dim 32, |dy|,|dx| bias, the map zero-padded
@@ -86,23 +85,6 @@ __global__ void sam_resize_norm_kernel(const uint8_t* __restrict__ mid, __half* 
 }
 
 // ------------------------------------------------------------------------------------------------------- convolutions
-__global__ void sam_im2col3x3_kernel(const __half* __restrict__ x, __half* __restrict__ col, int B, int H, int W, int C, int stride,
-                                     int Ho, int Wo, int ldk) {
-  const long long n = (long long)B * Ho * Wo * ldk;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const int k = (int)(i % ldk);
-    const long long r = i / ldk;
-    const int xo = (int)(r % Wo), yo = (int)((r / Wo) % Ho), b = (int)(r / ((long long)Wo * Ho));
-    __half v = __float2half_rn(0.f);
-    if (k < 9 * C) {
-      const int tap = k / C, c = k % C;
-      const int y = yo * stride - 1 + tap / 3, xx = xo * stride - 1 + tap % 3;
-      if (y >= 0 && y < H && xx >= 0 && xx < W) v = x[(((size_t)b * H + y) * W + xx) * C + c];
-    }
-    col[i] = v;
-  }
-}
-
 // d_w [9, C] (tap-major, BN folded), d_b [C]; NHWC in / out, fp16 or fp32 each.
 __global__ void sam_dwconv3x3_kernel(const void* __restrict__ in, int in_f32, const float* __restrict__ w, const float* __restrict__ bias,
                                      void* __restrict__ out, int out_f32, int B, int H, int W, int C, int stride, int Ho, int Wo,
@@ -427,16 +409,6 @@ extern "C" int vlfm_sam_preprocess(const uint8_t* d_img, uint8_t* d_mid, void* d
                                                                             v_first ? hksize : vksize, h_mean3[0], h_mean3[1], h_mean3[2],
                                                                             h_std3[0], h_std3[1], h_std3[2]);
   SAM_LAUNCHED("sam_resize_norm_kernel");
-  return VLFM_OK;
-}
-
-extern "C" int vlfm_sam_im2col3x3(const void* d_x16, void* d_col16, int B, int H, int W, int C, int stride, int ldk, void* stream) {
-  if (!d_x16 || !d_col16 || B < 1 || H < 1 || W < 1 || C < 1 || (stride != 1 && stride != 2) || ldk < 9 * C || (ldk & 7)) {
-    set_error("vlfm_sam_im2col3x3: bad argument"); return VLFM_E_INVALID; }
-  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
-  sam_im2col3x3_kernel<<<grid1d((long long)B * Ho * Wo * ldk, 256), 256, 0, (cudaStream_t)stream>>>(
-      (const __half*)d_x16, (__half*)d_col16, B, H, W, C, stride, Ho, Wo, ldk);
-  SAM_LAUNCHED("sam_im2col3x3_kernel");
   return VLFM_OK;
 }
 

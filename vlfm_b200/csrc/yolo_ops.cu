@@ -1,8 +1,8 @@
 // YOLOv7-E6E kernels (vlfm/vlm/yolov7.py YOLOv7.predict); the engine is vlfm_b200/vlm/yolov7_engine.py.  Activations are fp16
 // NHWC rows with a row stride (`ld*`, in elements), so a layer can read or write one channel slice of a concat buffer.  Every
-// conv is an im2col pass (3x3) or nothing (1x1) plus vlfm_gemm_f16 with VLFM_EPI_BIAS_SILU_F16; these kernels are the rest:
+// conv is vlfm_im2col_f16 (3x3) or nothing (1x1) plus vlfm_gemm_f16 with VLFM_EPI_BIAS_SILU_F16; these kernels are the rest:
 //   - yolo_preprocess: cv2 INTER_AREA resize of uint8 frames, /255 to fp16 and ReOrg (space-to-depth), one launch;
-//   - yolo_im2col3x3, yolo_maxpool2, yolo_spp_pools, yolo_upsample2, yolo_add: strided layer primitives;
+//   - yolo_maxpool2, yolo_spp_pools, yolo_upsample2, yolo_add: strided layer primitives;
 //   - yolo_decode, yolo_sort, yolo_nms, yolo_boxes: the IDetect decode with the confidence filter, the score order, greedy NMS
 //     and scale_coords, into fixed-size per-frame buffers so that the whole predict is one CUDA graph.
 // Nothing here uses atomics in a way that changes results: candidate compaction order is undone by the sort, whose key
@@ -68,29 +68,6 @@ yolo_preprocess_kernel(const uint8_t* __restrict__ img, __half* __restrict__ out
 }
 
 // ------------------------------------------------------------------------------------------------------------ layer ops
-// x [B,H,W,C] (row stride ldx) -> col [B*Ho*Wo, ldk]: 3x3, pad 1, stride 1 or 2, column (ky*3+kx)*C + c, columns >= 9C zero.
-// Eight channels per thread (C % 8 == 0, ldx % 8 == 0).
-__global__ void __launch_bounds__(256)
-yolo_im2col3x3_kernel(const __half* __restrict__ x, int ldx, __half* __restrict__ col, int B, int H, int W, int C, int stride,
-                      int Ho, int Wo, int ldk) {
-  const int c8 = ldk / 8;
-  const long long total = (long long)B * Ho * Wo * c8;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int q = (int)(i % c8);
-    const long long r = i / c8;
-    const int ox = (int)(r % Wo), oy = (int)((r / Wo) % Ho), b = (int)(r / ((long long)Wo * Ho));
-    uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    const int col0 = q * 8;
-    if (col0 < 9 * C) {
-      const int tap = col0 / C, c = col0 - tap * C;
-      const int iy = oy * stride - 1 + tap / 3, ix = ox * stride - 1 + tap % 3;
-      if ((unsigned)iy < (unsigned)H && (unsigned)ix < (unsigned)W)
-        v = *reinterpret_cast<const uint4*>(x + (((size_t)b * H + iy) * W + ix) * ldx + c);
-    }
-    *reinterpret_cast<uint4*>(col + r * ldk + col0) = v;
-  }
-}
-
 // MaxPool2d(2, 2): x [B,H,W,C] (ldx) -> out [B,H/2,W/2,C] (ldo)
 __global__ void yolo_maxpool2_kernel(const __half* __restrict__ x, int ldx, __half* __restrict__ out, int ldo, int B, int H, int W,
                                      int C, int Ho, int Wo) {
@@ -323,17 +300,6 @@ extern "C" int vlfm_yolo_preprocess(const uint8_t* d_img, void* d_out16, int B, 
   yolo_preprocess_kernel<<<yolo_grid((long long)B * OH * OW, 256), 256, 0, (cudaStream_t)stream>>>(
       d_img, (__half*)d_out16, B, H, W, OH, OW, d_yofs, d_ysi, d_ybeta, d_xofs, d_xsi, d_xalpha);
   YOLO_LAUNCHED("yolo_preprocess_kernel");
-  return VLFM_OK;
-}
-
-extern "C" int vlfm_yolo_im2col3x3(const void* d_x16, int ldx, void* d_col16, int B, int H, int W, int C, int stride, int ldk, void* stream) {
-  if (!d_x16 || !d_col16 || B < 1 || H < 1 || W < 1 || C < 8 || (C & 7) || ldx < C || (ldx & 7) || (stride != 1 && stride != 2) ||
-      ldk < 9 * C || (ldk & 7) || ((uintptr_t)d_x16 & 15) || ((uintptr_t)d_col16 & 15)) {
-    set_error("vlfm_yolo_im2col3x3: bad argument"); return VLFM_E_INVALID; }
-  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
-  yolo_im2col3x3_kernel<<<yolo_grid((long long)B * Ho * Wo * (ldk / 8), 256), 256, 0, (cudaStream_t)stream>>>(
-      (const __half*)d_x16, ldx, (__half*)d_col16, B, H, W, C, stride, Ho, Wo, ldk);
-  YOLO_LAUNCHED("yolo_im2col3x3_kernel");
   return VLFM_OK;
 }
 

@@ -1,10 +1,10 @@
 """The PointNav policy step on the library's kernels: depth in -> action, with each environment's hidden state and previous
 action updated in place.
 
-Encoder: every conv is an im2col pass (``vlfm_pointnav_depth_in`` for conv1, ``vlfm_sam_im2col3x3`` for the 3x3 convs,
-``vlfm_pointnav_gather_s2`` for the stride-2 1x1 downsamples) plus the wgmma GEMM (fp16 operands, fp32 out) through
-``vlm/dense.py``; each GroupNorm, with the block's residual add (identity, or the downsample's GroupNorm) and ReLU, is one
-``vlfm_pointnav_groupnorm`` launch on the fp32 GEMM output.  Recurrent part in fp32: ``visual_fc`` (weight columns permuted
+Encoder: every conv is an im2col pass (``vlfm_pointnav_depth_in`` for conv1, ``dense.im2col`` for the 3x3 convs and the
+stride-2 1x1 downsamples) plus the wgmma GEMM (fp16 operands, fp32 out) through ``vlm/dense.py``; each GroupNorm, with the
+block's residual add (identity, or the downsample's GroupNorm) and ReLU, is one ``vlfm_pointnav_groupnorm`` launch on the fp32
+GEMM output.  Recurrent part in fp32: ``visual_fc`` (weight columns permuted
 from the NCHW flatten to NHWC), the two LSTM gate GEMMs ([x | h] @ [W_ih | W_hh]^T + b_ih + b_hh) on
 ``vlfm_pointnav_gemv_f32``, the cells and the head on ``vlfm_pointnav_lstm_*``.
 
@@ -20,7 +20,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from .. import _lib
-from ..vlm.dense import gemm_f16
+from ..vlm.dense import conv_rows, gemm_f16, im2col
 from .pointnav_weights import BACKBONE, EMB, HEAD_CONTINUOUS, HEAD_DISCRETE, HID, NGROUPS, STAGES, VIS
 
 F16, F32 = torch.float16, torch.float32
@@ -52,14 +52,6 @@ def spatial_plan(hw: Tuple[int, int]) -> List[Tuple[int, int]]:
     return sizes
 
 
-def conv_rows(w: torch.Tensor) -> torch.Tensor:
-    """[O, C, k, k] -> [O, ldk] fp16 GEMM rows with columns (ky, kx, c), K zero-padded to a multiple of 8."""
-    O, C, k, _ = w.shape
-    r = w.permute(0, 2, 3, 1).reshape(O, k * k * C)
-    ldk = (k * k * C + 7) // 8 * 8
-    return torch.nn.functional.pad(r, (0, ldk - r.shape[1])).to(F16).contiguous()
-
-
 class PointNavEngine:
     def __init__(self, w: Dict[str, torch.Tensor], discrete: bool, max_batch: int = 1, input_hw: Tuple[int, int] = (224, 224),
                  num_envs: Optional[int] = None, device="cuda", use_graph: bool = True) -> None:
@@ -78,7 +70,7 @@ class PointNavEngine:
         self.w: Dict[str, torch.Tensor] = {}
         for k, v in w.items():
             if v.dim() == 4:
-                self.w[k] = conv_rows(v).to(dev)
+                self.w[k] = conv_rows(v).to(dev, F16)
             elif not k.startswith("net.state_encoder.") and k != "net.visual_fc.1.weight":
                 self.w[k] = f(v)
         # visual_fc over the NHWC flatten: column (y*4 + x)*128 + c holds the reference's column c*16 + y*4 + x
@@ -139,8 +131,8 @@ class PointNavEngine:
         _lib.check(rc, "vlfm_pointnav_groupnorm")
 
     def _im2col(self, x16, B, H, W, C, stride):
-        rc = self.lib.vlfm_sam_im2col3x3(x16.data_ptr(), self.col.data_ptr(), B, H, W, C, stride, 9 * C, _lib.stream_ptr())
-        _lib.check(rc, "vlfm_sam_im2col3x3")
+        Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+        im2col(x16[:B * H * W * C].view(-1, C), B, H, W, 3, stride, self.col[:B * Ho * Wo * 9 * C].view(-1, 9 * C))
 
     def _gemv(self, x, ldx, wname, bname, y, ldy, B, N, K, relu):
         rc = self.lib.vlfm_pointnav_gemv_f32(x.data_ptr(), ldx, self.w[wname].data_ptr(), self.w[wname].shape[1], self.w[bname].data_ptr(),
@@ -173,7 +165,7 @@ class PointNavEngine:
                 self._im2col(self.t16, B, ho, wo, c, 1)
                 self._gemm(self.col, M, 9 * c, p + "convs.3.weight", self.t32, c)
                 if p + "downsample.0.weight" in self.w:
-                    _lib.check(self.lib.vlfm_pointnav_gather_s2(self.x16.data_ptr(), self.g16.data_ptr(), B, h, w, ci, st), "vlfm_pointnav_gather_s2")
+                    im2col(self.x16[:B * h * w * ci].view(-1, ci), B, h, w, 1, 2, self.g16[:M * ci].view(M, ci))
                     self._gemm(self.g16, M, ci, p + "downsample.0.weight", self.d32, c)
                     self._gn(self.t32, p + "convs.4", B, ho * wo, c, NGROUPS, rmode=2, y=self.d32, name_b=p + "downsample.1",
                              out32=self.x32, out16=self.x16)

@@ -1,5 +1,5 @@
-"""Torch-tensor wrappers over the dense C-ABI entry points (csrc/gemm_wgmma.cu, vit_ops.cu, gdino_ops.cu): the only Python code
-that calls them.  Every engine (BLIP-2, Swin, GroundingDINO, MobileSAM) goes through these.
+"""Torch-tensor wrappers over the dense C-ABI entry points (csrc/gemm_wgmma.cu, vit_ops.cu, gdino_ops.cu, im2col.cu): the only
+Python code that calls them.  Every engine (BLIP-2, Swin, GroundingDINO, MobileSAM, PointNav, YOLOv7) goes through these.
 
 Each wrapper writes into the outputs the caller gives and allocates a required output only when it is not given, so a CUDA-graph
 captured forward can pass preallocated buffers.  An optional output of the ABI (a NULL pointer there) is left out by passing
@@ -149,3 +149,23 @@ def cast_addpos_f16(x: Tensor, pos: Optional[Tensor], out: Optional[Tensor] = No
     rc = _lib.load().vlfm_cast_addpos_f16(x.data_ptr(), _lib.ptr(pos), _lib.ptr(out), out_pos.data_ptr(), x.numel(), _lib.stream_ptr())
     _lib.check(rc, "vlfm_cast_addpos_f16")
     return out_pos
+
+
+def im2col(x: Tensor, B: int, H: int, W: int, k: int, stride: int, out: Optional[Tensor] = None) -> Tensor:
+    """Rows of a k x k conv (pad k // 2) over x [B*H*W, C] NHWC rows -> out [B*Ho*Wo, ldk] (contiguous), the A operand of a GEMM
+    with the weight ``conv_rows(w)``.  A new ``out`` has ldk = k*k*C rounded up to a multiple of 8."""
+    C = x.shape[1]
+    if out is None:
+        Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+        out = torch.empty((B * Ho * Wo, (k * k * C + 7) // 8 * 8), dtype=F16, device=x.device)
+    rc = _lib.load().vlfm_im2col_f16(x.data_ptr(), x.stride(0), out.data_ptr(), B, H, W, C, k, stride, out.shape[1], _lib.stream_ptr())
+    _lib.check(rc, "vlfm_im2col_f16")
+    return out
+
+
+def conv_rows(w: Tensor) -> Tensor:
+    """Conv weight [O, C, k, k] -> GEMM rows [O, ldk] in w's dtype, columns (ky, kx, c) zero-padded to ldk = k*k*C rounded up to a
+    multiple of 8: the column order of ``im2col``."""
+    O, C, k, _ = w.shape
+    r = w.permute(0, 2, 3, 1).reshape(O, k * k * C)
+    return torch.nn.functional.pad(r, (0, (k * k * C + 7) // 8 * 8 - k * k * C)).contiguous()

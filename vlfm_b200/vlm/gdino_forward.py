@@ -30,6 +30,8 @@ from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
+from .dense import conv_rows
+
 
 class GdinoForward:
     def __init__(self, model, ops, backbone=None) -> None:
@@ -50,13 +52,8 @@ class GdinoForward:
         self.neck: List[Dict[str, torch.Tensor]] = []
         for lvl, seq in enumerate(core.input_proj_vision):
             conv, gn = seq[0], seq[1]
-            w = conv.weight.detach()
-            if conv.kernel_size == (1, 1):
-                w2 = w.reshape(w.shape[0], w.shape[1])
-            else:   # [out, in, 3, 3] -> [out, (ky, kx, in)]: the im2col row order
-                w2 = w.permute(0, 2, 3, 1).reshape(w.shape[0], -1)
-            self.neck.append(dict(w=ops.weight(w2), b=conv.bias.detach().float().contiguous(), g=gn.weight.detach().float().contiguous(),
-                                  be=gn.bias.detach().float().contiguous(), groups=gn.num_groups, eps=gn.eps, k=conv.kernel_size[0]))
+            self.neck.append(dict(w=ops.weight(conv_rows(conv.weight.detach())), b=conv.bias.detach().float().contiguous(),
+                                  g=gn.weight.detach().float().contiguous(), be=gn.bias.detach().float().contiguous(), groups=gn.num_groups, eps=gn.eps, k=conv.kernel_size[0]))
         self.enc_out_w = ops.weight(core.enc_output.weight.detach())
         self.enc_out_b = core.enc_output.bias.detach().float().contiguous()
         self.enc_norm = (core.enc_output_norm.weight.detach().float().contiguous(), core.enc_output_norm.bias.detach().float().contiguous(),
@@ -174,11 +171,10 @@ class GdinoForward:
             nk = self.neck[lvl]
             h, w = shapes[lvl]
             if nk["k"] == 1:
-                rows = feats[lvl][0]
-                a = ops.to_operand(rows)
-            else:
-                rows4, hh, ww = feats[-1]
-                a = ops.im2col3x3s2(rows4, B, hh, ww)
+                a = last16 = ops.to_operand(feats[lvl][0])
+            else:   # the 3x3 stride-2 conv reads the last backbone stage, whose fp16 operand level 2 has just made
+                _, hh, ww = feats[-1]
+                a = ops.im2col3x3s2(last16, B, hh, ww)
             y = ops.linear_operand(a, nk["w"], nk["b"])                                     # [B*h*w, 256] fp32
             ops.groupnorm_rows(y, B, h * w, d, nk["groups"], nk["g"], nk["be"], nk["eps"], src, sc["offsets"][lvl], S)
         # ---- encoder: GroundingDinoEncoder.forward is a loop over its layers; the per-call constants it rebuilds -- the deformable

@@ -7,7 +7,7 @@ from typing import Optional
 import torch
 
 from .. import _lib
-from .dense import cast_f16, gemm_f16, layernorm as _layernorm
+from .dense import cast_f16, gemm_f16, im2col, layernorm as _layernorm
 
 F16, F32 = torch.float16, torch.float32
 
@@ -37,11 +37,8 @@ class LibOps:
 
     # ---- neck
     def im2col3x3s2(self, rows: torch.Tensor, B: int, h: int, w: int) -> torch.Tensor:
-        C = rows.shape[1]
-        ho, wo = (h + 2 - 3) // 2 + 1, (w + 2 - 3) // 2 + 1
-        col = torch.empty((B * ho * wo, 9 * C), dtype=F16, device=rows.device)
-        _lib.check(self.lib.vlfm_im2col3x3s2(rows.data_ptr(), col.data_ptr(), B, h, w, C, _lib.stream_ptr()), "vlfm_im2col3x3s2")
-        return col
+        """Rows of the fourth level's 3x3 stride-2 conv; fp32 rows are cast to the fp16 operand first."""
+        return im2col(self.to_operand(rows), B, h, w, 3, 2)
 
     def groupnorm_rows(self, y: torch.Tensor, B: int, HW: int, C: int, groups: int, g: torch.Tensor, b: torch.Tensor, eps: float,
                        out: torch.Tensor, row_off: int, S: int) -> None:

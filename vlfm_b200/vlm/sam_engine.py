@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from .. import _lib
-from .dense import attention_f16, gemm_f16, gemm_f16_resid_ln, layernorm
+from .dense import attention_f16, gemm_f16, gemm_f16_resid_ln, im2col, layernorm
 from .preprocess import bilinear_tables, pillow_vertical_first
 from .sam_config import SamDims
 
@@ -87,10 +87,6 @@ class MobileSamEngine:
         rc = self.lib.vlfm_sam_add_act(a.data_ptr(), _lib.ptr(b), _lib.ptr(out32), _lib.ptr(out16), n, gelu, _lib.stream_ptr())
         _lib.check(rc, "vlfm_sam_add_act")
 
-    def _im2col(self, x, col, B, H, W, C, stride):
-        rc = self.lib.vlfm_sam_im2col3x3(x.data_ptr(), col.data_ptr(), B, H, W, C, stride, col.shape[1], _lib.stream_ptr())
-        _lib.check(rc, "vlfm_sam_im2col3x3")
-
     # ------------------------------------------------------------------------------------------------------- encoder
     def _tables(self, H: int, W: int):
         S = self.d.img_size
@@ -148,12 +144,12 @@ class MobileSamEngine:
         # stem: conv3x3 s2 (3 -> E0/2) + GELU, conv3x3 s2 (E0/2 -> E0)
         h1 = S // 2
         col = v(A, B * h1 * h1, self.w["stem0.w"].shape[1])
-        self._im2col(x0, col, B, S, S, 3, 2)
+        im2col(x0.view(-1, 3), B, S, S, 3, 2, col)
         s0 = v(Bb, B * h1 * h1, d.stem_mid)
         gemm_f16(col, *self._wb("stem0"), _lib.EPI_BIAS_GELU_F16, s0)
         n0 = B * r[0] * r[0]
         col = v(A, n0, self.w["stem1.w"].shape[1])
-        self._im2col(s0, col, B, h1, h1, d.stem_mid, 2)
+        im2col(s0, B, h1, h1, 3, 2, col)
         x32, y32, z32, x16 = v(bf["x32"], n0, E[0]), v(bf["y32"], n0, E[0]), v(bf["z32"], n0, E[0]), v(bf["x16"], n0, E[0])
         gemm_f16(col, *self._wb("stem1"), _lib.EPI_BIAS_F32, x32)
         self._add_act(x32, None, None, x16, x32.numel(), 0)
@@ -202,7 +198,7 @@ class MobileSamEngine:
         t16 = v(Bb, n, P)
         layernorm(t32, *self._wb("neck1"), 1e-6, t16)
         col = v(A, n, self.w["neck2.w"].shape[1])
-        self._im2col(t16, col, B, R, R, P, 1)
+        im2col(t16, B, R, R, 3, 1, col)
         gemm_f16(col, *self._wb("neck2"), _lib.EPI_BIAS_F32, t32)
         out = self.emb[:B].view(n, P)
         layernorm(t32, *self._wb("neck3"), 1e-6, out32=out)

@@ -1,8 +1,8 @@
 """mobile_sam checkpoint names -> the layout of ``sam_engine.MobileSamEngine``.
 
 - Every ``Conv2d_BN`` (conv + eval-mode BatchNorm, eps 1e-5) is folded into one weight and bias.
-- Convolutions become GEMM operands: 1x1 -> [O, C]; 3x3 -> [O, ldk] with columns (ky, kx, c), K zero-padded to a multiple of 8
-  (the stem's 27 -> 32); depthwise 3x3 -> [9, C] (tap-major) for ``vlfm_sam_dwconv3x3``.
+- Convolutions become GEMM operands: 1x1 -> [O, C]; 3x3 -> ``dense.conv_rows``, K zero-padded to a multiple of 8 (the stem's
+  27 -> 32); depthwise 3x3 -> [9, C] (tap-major) for ``vlfm_sam_dwconv3x3``.
 - The TinyViT qkv rows, interleaved per head (q_h, k_h, v_h), are permuted to [q | k | v] with head h at h*32 inside each, and
   ``attention_biases[h, idx]`` is re-indexed by |dy|*ws + |dx|.
 - The 2x2 stride-2 transposed convs become GEMMs with rows (dy, dx, o).
@@ -19,6 +19,7 @@ from typing import Dict
 
 import torch
 
+from .dense import conv_rows
 from .sam_config import SamDims
 
 BN_EPS = 1e-5
@@ -52,14 +53,6 @@ def fold_conv_bn(sd: Dict[str, torch.Tensor], name: str):
     mu, var = sd[name + ".bn.running_mean"].double(), sd[name + ".bn.running_var"].double()
     s = g / torch.sqrt(var + BN_EPS)
     return (w * s[:, None, None, None]).float(), (b - mu * s).float()
-
-
-def conv3x3_rows(w: torch.Tensor) -> torch.Tensor:
-    """[O, C, 3, 3] -> [O, ldk] GEMM rows with columns (ky, kx, c), ldk = 9C rounded up to a multiple of 8."""
-    O, C = w.shape[:2]
-    r = w.permute(0, 2, 3, 1).reshape(O, 9 * C)
-    ldk = (9 * C + 7) // 8 * 8
-    return torch.nn.functional.pad(r, (0, ldk - 9 * C)).contiguous()
 
 
 def convT_rows(w: torch.Tensor, b: torch.Tensor):
@@ -102,7 +95,7 @@ def convert_state_dict(sd: Dict[str, torch.Tensor], d: SamDims) -> Dict[str, tor
     E = d.embed_dims
     for i, name in enumerate(("patch_embed.seq.0", "patch_embed.seq.2")):
         w, b = cbn(e + name)
-        out[f"stem{i}.w"], out[f"stem{i}.b"] = conv3x3_rows(w), b
+        out[f"stem{i}.w"], out[f"stem{i}.b"] = conv_rows(w), b
     for s in range(len(E)):
         p = f"{e}layers.{s}."
         for bi in range(d.depths[s]):
@@ -134,7 +127,7 @@ def convert_state_dict(sd: Dict[str, torch.Tensor], d: SamDims) -> Dict[str, tor
             put_1x1(f"l{s}.down.conv3", p + "downsample.conv3")
     out["neck0.w"] = g(e + "neck.0.weight").reshape(d.prompt_dim, E[-1]).contiguous()
     put_ln("neck1", e + "neck.1")
-    out["neck2.w"] = conv3x3_rows(g(e + "neck.2.weight"))
+    out["neck2.w"] = conv_rows(g(e + "neck.2.weight"))
     put_ln("neck3", e + "neck.3")
 
     pe = "prompt_encoder."

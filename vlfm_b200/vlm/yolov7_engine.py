@@ -3,8 +3,8 @@ CUDA graph per (B, H, W) for preprocess + network + decode + NMS + box mapping.
 
 Activations are fp16 NHWC rows.  A layer whose output feeds a Concat writes straight into its channel slice of the concat's
 buffer (GEMM ``ldo``, strided pools / upsample / add), so no Concat copies anything.  1x1 convs are GEMMs on the rows, 3x3 convs
-``vlfm_yolo_im2col3x3`` (strided: its input may be a slice) plus the GEMM, all with the folded BatchNorm in the bias and SiLU in
-the epilogue.  Thresholds and the class filter sit in a device parameter block, so changing them does not re-capture.
+``dense.im2col`` (its input may be a slice) plus the GEMM, all with the folded BatchNorm in the bias and SiLU in the epilogue.
+Thresholds and the class filter sit in a device parameter block, so changing them does not re-capture.
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from .. import _lib
-from .dense import gemm_f16
+from .dense import conv_rows, gemm_f16, im2col
 from .yolov7_weights import Layer, fold, fold_detect
 
 F16 = torch.float16
@@ -92,13 +92,6 @@ class YoloEngine:
         self.set_params(0.25, 0.45, None, False)
 
     # --------------------------------------------------------------------------------------------------------- weights
-    def _gemm_weight(self, w: torch.Tensor, cin_pad: Optional[int] = None) -> torch.Tensor:
-        o, i, k, _ = w.shape
-        w = w.permute(0, 2, 3, 1)                                   # (o, ky, kx, c): im2col column order
-        if cin_pad and cin_pad > i:
-            w = torch.nn.functional.pad(w, (0, cin_pad - i))
-        return w.reshape(o, -1).to(self.dev, F16).contiguous()
-
     def _fold_weights(self) -> None:
         self.w: Dict[Tuple[int, str], Tuple[torch.Tensor, torch.Tensor, int, int]] = {}
         det = self.layers[-1]
@@ -109,8 +102,9 @@ class YoloEngine:
                     wf, bf = fold_detect(c, det.extra["ia"][k], det.extra["im"][k])
                 else:
                     wf, bf = fold(c)
-                pad = 16 if (l.type == "Conv" and wf.shape[1] == 12 and l.f[0] >= 0 and self._is_reorg(l.f[0])) else None
-                self.w[(l.i, name)] = (self._gemm_weight(wf, pad), bf.to(self.dev, torch.float32).contiguous(), wf.shape[2], c.stride)
+                if l.type == "Conv" and wf.shape[1] == 12 and l.f[0] >= 0 and self._is_reorg(l.f[0]):
+                    wf = torch.nn.functional.pad(wf, (0, 0, 0, 0, 0, 4))      # ReOrg's map: 12 channels + 4 zero
+                self.w[(l.i, name)] = (conv_rows(wf).to(self.dev, F16), bf.to(self.dev, torch.float32).contiguous(), wf.shape[2], c.stride)
         self.anchors = det.extra["anchors"].to(self.dev, torch.float32).reshape(-1, self.na, 2).contiguous()
         self.strides = [float(s) for s in det.extra["strides"]]
 
@@ -284,12 +278,9 @@ class YoloEngine:
         if k == 1:
             gemm_f16(x, wt, b, epi, out=out)
             return
-        C_ = x.shape[1]
         ho, wo = (h - 1) // s + 1, (w - 1) // s + 1
-        M, K = B * ho * wo, 9 * C_
-        col = bufs["col"][:M * K].view(M, K)
-        _lib.check(self.lib.vlfm_yolo_im2col3x3(x.data_ptr(), x.stride(0), col.data_ptr(), B, h, w, C_, s, K, _lib.stream_ptr()),
-                   "vlfm_yolo_im2col3x3")
+        M, K = B * ho * wo, wt.shape[1]
+        col = im2col(x, B, h, w, 3, s, bufs["col"][:M * K].view(M, K))
         gemm_f16(col, wt, b, epi, out=out)
 
     def _tmp(self, bufs, n: int, rows: int, c: int) -> torch.Tensor:
