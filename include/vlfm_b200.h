@@ -193,7 +193,12 @@ int vlfm_preprocess_im2col(const uint8_t* d_img, uint8_t* d_mid, void* d_out, in
 /* x[b,0] = cls + pos[0]; x[b,1+p] = patch[b,p] + pos[1+p]   (fp32; ViT token assembly) */
 int vlfm_assemble_tokens(const float* d_patch, const float* d_cls, const float* d_pos, float* d_x, int B,
                          int T, int D, void* stream);
-/* LayerNorm over the last dimension: fp32 in, fp16 (d_out16) and/or fp32 (d_out32) out. */
+/* LayerNorm over the last dimension: fp32 in, fp16 (d_out16) and/or fp32 (d_out32) out.
+ * Every LayerNorm entry point (vlfm_layernorm, vlfm_layernorm_x2, vlfm_layernorm_reduce(_x2) and the resid-LN GEMMs, whose D is N):
+ *   - D <= 1536, and D, ldx, ldo16, ldo32 multiples of 4, else VLFM_E_UNSUPPORTED (the resid-LN GEMMs return VLFM_E_INVALID for
+ *     a D or stride that is not a multiple of 4, as for their other strides);
+ *   - d_x, d_gamma, d_beta, d_out32 and the partials 16-byte aligned, the fp16 outputs 8-byte aligned, else VLFM_E_INVALID.
+ * These are checked before anything is launched: a refused resid-LN call leaves x and the workspace untouched. */
 int vlfm_layernorm(const float* d_x, const float* d_gamma, const float* d_beta, void* d_out16, float* d_out32,
                    int rows, int D, int ldx, int ldo16, int ldo32, float eps, void* stream);
 /* softmax(scale * Q K^T) V per (batch, head); fp16 in/out, fp32 accumulate.

@@ -181,7 +181,11 @@ def test_attention_f16_argument_errors():
     assert L.launch_count() == n0 + 1
 
 
-@pytest.mark.parametrize("rows,D,eps", [(257, 1408, 1e-6), (32, 768, 1e-12), (19200, 96, 1e-5), (5, 1536, 1e-5), (100, 64, 1e-5)])
+# D = 4, 256 / 260, 768 / 772, 1536: both sides of the <2> / <6> / <12> float4-per-lane instantiations of layernorm_kernel;
+# rows = 1, 3, 5 around its four rows per block
+@pytest.mark.parametrize("rows,D,eps", [(257, 1408, 1e-6), (32, 768, 1e-12), (19200, 96, 1e-5), (5, 1536, 1e-5), (100, 64, 1e-5),
+                                        (1, 4, 1e-5), (5, 4, 1e-5), (3, 256, 1e-5), (1, 260, 1e-5), (5, 768, 1e-6), (3, 772, 1e-6),
+                                        (1, 1536, 1e-5), (3, 1536, 1e-6)])
 def test_layernorm_matches_torch(rows, D, eps):
     from vlfm_b200.vlm.dense import layernorm
 
@@ -193,3 +197,17 @@ def test_layernorm_matches_torch(rows, D, eps):
     ref = torch.nn.functional.layer_norm(x, (D,), gamma, beta, eps)
     assert (o32 - ref).abs().max().item() <= 2e-5
     assert (o16.float() - ref).abs().max().item() <= 4e-3
+    # the same rows as column windows of wider buffers (ldx, ldo16, ldo32 = D + 12, a spare row below): the same bits, and every
+    # spare element of x (NaN) stays unread and every spare element of the outputs keeps its payload-NaN bits
+    ld = D + 12
+    win = (slice(0, rows), slice(4, 4 + D))
+    xb = torch.full((rows + 1, ld), float("nan"), device="cuda")
+    xb[win] = x
+    o16b = torch.full((rows + 1, ld), NAN16, dtype=torch.int16, device="cuda")
+    o32b = torch.full((rows + 1, ld), 0x7FC05A5A, dtype=torch.int32, device="cuda")
+    layernorm(xb[win], gamma, beta, eps, o16b.view(torch.float16)[win], o32b.view(torch.float32)[win])
+    torch.cuda.synchronize()
+    assert torch.equal(o16b[win], o16.view(torch.int16)) and torch.equal(o32b[win], o32.view(torch.int32))
+    spare = torch.ones(rows + 1, ld, dtype=torch.bool, device="cuda")
+    spare[win] = False
+    assert bool((o16b[spare] == NAN16).all()) and bool((o32b[spare] == 0x7FC05A5A).all())

@@ -74,6 +74,12 @@ struct SplitK {
   __host__ __device__ __forceinline__ int sk_owner(int it) const { return (int)(((long long)(it + 1) * ctas - 1) / ((long long)tiles * num_k)); }
 };
 
+// LayerNorm rows (vit_ops.cu): at most LN_DMAX columns (layernorm_kernel<12>: 12 float4 per lane; layernorm_reduce_kernel: one
+// float4 per thread of at most 384).  layernorm_check: the argument checks of every LayerNorm entry point, resid-LN GEMMs included.
+constexpr int LN_DMAX = 1536;
+int layernorm_check(const char* who, const float* d_x, const float* d_gamma, const float* d_beta, const void* d_out16, const void* d_out16_lo,
+                    const float* d_out32, int D, int ldx, int ldo16, int ldo32);
+
 __device__ __forceinline__ float ld_cg_f32(const float* p) { return __ldcg(p); }
 __device__ __forceinline__ uint32_t ld_cg_u32(const uint32_t* p) { return __ldcg(p); }
 

@@ -1116,11 +1116,14 @@ extern "C" int vlfm_gemm_f16_resid_ln(const void* d_A, const void* d_W, const fl
     set_error("vlfm_gemm_f16_resid_ln: bad argument"); return VLFM_E_INVALID; }
   if ((K & 7) || (lda & 7) || (ldw & 7) || (ldx & 7) || (N & 3) || (ld16 & 3) || (ld32 & 3) || ((uintptr_t)d_A & 15) || ((uintptr_t)d_W & 15) ||
       ((uintptr_t)d_x & 15) || ((uintptr_t)d_partials & 15)) { set_error("vlfm_gemm_f16_resid_ln: alignment (K, strides %% 8; N %% 4; 16-byte pointers)"); return VLFM_E_INVALID; }
+  // the LayerNorm's own limits, before the GEMM changes x or the workspace
+  int rc = layernorm_check("vlfm_gemm_f16_resid_ln", d_x, d_gamma, d_beta, d_out16, nullptr, d_out32, N, ldx, ld16, ld32);
+  if (rc) return rc;
   GemmArgs g{d_bias, d_x, M, N, K, ldx, VLFM_EPI_BIAS_RESID_F32, (K + BK - 1) / BK, 0, nullptr, 0, 0, 0, nullptr, BM};
   SplitK layout;
   // a workspace means the caller allows a split K, which includes the cluster split (MobileSAM passes none: its rows' bits must
   // not depend on M)
-  int rc = gemm_dispatch(d_A, d_W, M, N, K, lda, ldw, g, stream, d_partials, partial_bytes, &layout, d_partials != nullptr);
+  rc = gemm_dispatch(d_A, d_W, M, N, K, lda, ldw, g, stream, d_partials, partial_bytes, &layout, d_partials != nullptr);
   if (rc) return rc;
   if (layout.splits != 1) return layernorm_reduce_impl(d_x, d_partials, layout, d_gamma, d_beta, d_out16, nullptr, d_out32, M, N, ldx, ld16, ld32, eps, stream);
   return vlfm_layernorm(d_x, d_gamma, d_beta, d_out16, d_out32, M, N, ldx, ld16, ld32, eps, stream);
@@ -1208,6 +1211,8 @@ extern "C" int vlfm_gemm_f16x2_resid_ln(const void* d_A_hi, const void* d_A_lo, 
   if (rc) return rc;
   if (!d_gamma || !d_beta || !d_out_hi || !d_out_lo || (N & 3) || (ld16 & 3) || (ld32 & 3) || ((uintptr_t)d_partials & 15)) {
     set_error("vlfm_gemm_f16x2_resid_ln: bad argument / alignment"); return VLFM_E_INVALID; }
+  rc = layernorm_check("vlfm_gemm_f16x2_resid_ln", d_x, d_gamma, d_beta, d_out_hi, d_out_lo, d_out32, N, ldx, ld16, ld32);
+  if (rc) return rc;
   GemmArgs g{d_bias, d_x, M, N, K, ldx, VLFM_EPI_BIAS_RESID_F32, (K + BK - 1) / BK, 0, nullptr, 0, 0, 0, nullptr, BM};
   int splits = 1;
   rc = gemm_x2_dispatch(d_A_hi, d_A_lo, d_W_hi, d_W_lo, M, N, K, lda, ldw, g, stream, d_partials, partial_bytes, &splits);

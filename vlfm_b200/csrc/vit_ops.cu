@@ -657,20 +657,33 @@ extern "C" int vlfm_assemble_tokens(const float* d_patch, const float* d_cls, co
   return VLFM_OK;
 }
 
+namespace vlfm {
+// The shape and alignment both LayerNorm kernels need, checked before anything launches (the resid-LN GEMMs run it before their
+// GEMM, so a refused call leaves x and the workspace as they were).  D <= 1536; D and the strides multiples of 4; x, gamma, beta
+// and out32 read / written as float4 (16-byte aligned), out16 and out_lo as 4 halves (8-byte aligned).  Null outputs are skipped.
+int layernorm_check(const char* who, const float* d_x, const float* d_gamma, const float* d_beta, const void* d_out16, const void* d_out16_lo,
+                    const float* d_out32, int D, int ldx, int ldo16, int ldo32) {
+  if (D > LN_DMAX) { set_error("%s: D=%d too large (max %d)", who, D, LN_DMAX); return VLFM_E_UNSUPPORTED; }
+  if ((D & 3) || (ldx & 3) || (ldo16 & 3) || (ldo32 & 3)) { set_error("%s: D and strides must be multiples of 4", who); return VLFM_E_UNSUPPORTED; }
+  if (((uintptr_t)d_x & 15) || ((uintptr_t)d_gamma & 15) || ((uintptr_t)d_beta & 15) || ((uintptr_t)d_out32 & 15) ||
+      ((uintptr_t)d_out16 & 7) || ((uintptr_t)d_out16_lo & 7)) {
+    set_error("%s: x, gamma, beta, out32 must be 16-byte aligned, the fp16 outputs 8-byte aligned", who); return VLFM_E_INVALID; }
+  return VLFM_OK;
+}
+}  // namespace vlfm
+
 static int layernorm_impl(const float* d_x, const float* d_gamma, const float* d_beta, void* d_out16, void* d_out16_lo, float* d_out32,
                           int rows, int D, int ldx, int ldo16, int ldo32, float eps, void* stream) {
   __half* lo16 = (__half*)d_out16_lo;
   if (!d_x || !d_gamma || !d_beta || (!d_out16 && !d_out32) || rows < 1 || D < 1) { set_error("vlfm_layernorm: bad argument"); return VLFM_E_INVALID; }
+  if (int rc = layernorm_check("vlfm_layernorm", d_x, d_gamma, d_beta, d_out16, d_out16_lo, d_out32, D, ldx, ldo16, ldo32)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  dim3 grid((rows + 7) / 8);
+  const dim3 grid((rows + 3) / 4);
   cudaError_t e;
   __half* o16 = (__half*)d_out16;
-  if ((D & 3) || (ldx & 3) || (ldo16 & 3) || (ldo32 & 3)) { set_error("vlfm_layernorm: D and strides must be multiples of 4"); return VLFM_E_UNSUPPORTED; }
-  grid = dim3((rows + 3) / 4);
   if (D <= 128 * 2) e = launch_pdl(layernorm_kernel<2>, grid, dim3(128), 0, st, d_x, d_gamma, d_beta, o16, d_out32, rows, D, ldx, ldo16, ldo32, eps, lo16);
   else if (D <= 128 * 6) e = launch_pdl(layernorm_kernel<6>, grid, dim3(128), 0, st, d_x, d_gamma, d_beta, o16, d_out32, rows, D, ldx, ldo16, ldo32, eps, lo16);
-  else if (D <= 128 * 12) e = launch_pdl(layernorm_kernel<12>, grid, dim3(128), 0, st, d_x, d_gamma, d_beta, o16, d_out32, rows, D, ldx, ldo16, ldo32, eps, lo16);
-  else { set_error("vlfm_layernorm: D=%d too large (max 1536)", D); return VLFM_E_UNSUPPORTED; }
+  else e = launch_pdl(layernorm_kernel<12>, grid, dim3(128), 0, st, d_x, d_gamma, d_beta, o16, d_out32, rows, D, ldx, ldo16, ldo32, eps, lo16);
   { int rc = check_cuda(e, "layernorm_kernel"); if (rc) return rc; }
   count_launch();
   return VLFM_OK;
@@ -694,12 +707,13 @@ int layernorm_reduce_impl(float* d_x, const float* d_partials, const SplitK& sk,
   if (!d_x || !d_partials || !d_gamma || !d_beta || (!d_out16 && !d_out32) || rows < 1 || D < 1 || sk.splits < 0 || sk.splits > 16 ||
       (sk.splits == 0 && (sk.ctas < 1 || sk.row_tiles < 1 || sk.tiles != sk.row_tiles * ((D + SK_TILE - 1) / SK_TILE) || sk.num_k < 1))) {
     set_error("vlfm_layernorm_reduce: bad argument"); return VLFM_E_INVALID; }
-  if ((D & 3) || (ldx & 3) || (ldo16 & 3) || (ldo32 & 3) || (sk.stride & 3)) { set_error("vlfm_layernorm_reduce: D and strides must be multiples of 4"); return VLFM_E_UNSUPPORTED; }
+  if (int rc = layernorm_check("vlfm_layernorm_reduce", d_x, d_gamma, d_beta, d_out16, d_out16_lo, d_out32, D, ldx, ldo16, ldo32)) return rc;
+  if (sk.stride & 3) { set_error("vlfm_layernorm_reduce: D and strides must be multiples of 4"); return VLFM_E_UNSUPPORTED; }
+  if ((uintptr_t)d_partials & 15) { set_error("vlfm_layernorm_reduce: partials must be 16-byte aligned"); return VLFM_E_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   const dim3 grid(rows);
   __half* o16 = (__half*)d_out16;
   cudaError_t e;
-  if (D > 1536) { set_error("vlfm_layernorm_reduce: D=%d too large (max 1536)", D); return VLFM_E_UNSUPPORTED; }
   const int threads = (((D >> 2) + 31) / 32) * 32;
   e = launch_pdl(layernorm_reduce_kernel, grid, dim3(threads), 0, st, d_x, d_partials, sk, d_gamma, d_beta, o16, d_out32, rows, D, ldx, ldo16, ldo32, eps, lo16);
   { int rc = check_cuda(e, "layernorm_reduce_kernel"); if (rc) return rc; }
