@@ -14,7 +14,8 @@
  *   - batched: `batch` environments per call; env b uses grid slot
  *     d_slot[b] (or b when d_slot == NULL) of the [nslots, G, G(, C)] state tensors.
  *   - per-environment soft errors (camera off-grid, scatter out of range) are
- *     reported through `d_status[b]` bit flags (VLFM_ST_*), read by the host at its
+ *     reported through `d_status` bit flags (VLFM_ST_*; each entry point says whether
+ *     d_status is indexed by call row or by grid slot), read by the host at its
  *     next synchronisation point and turned into the reference's exceptions.
  */
 #ifndef VLFM_B200_H_
@@ -81,7 +82,8 @@ int vlfm_value_workspace_bytes(const VlfmValueParams* p, int batch, size_t* byte
  * d_explored [nslots, G, G]  uint8 or NULL (value_map.py:369-375 masking of the new
  *                            observation; the full-grid part is vlfm_value_mask_unexplored)
  * d_workspace                vlfm_value_workspace_bytes(), must be zero-filled once
- * d_status [batch]           int32, OR-ed with VLFM_ST_* flags                        */
+ * d_status [nslots]          int32: row b ORs its VLFM_ST_* flags into d_status[slot of row b], so the
+ *                            flags of a slot stay with its grids until the host clears them */
 int vlfm_value_update(const VlfmValueParams* p, int batch, const int32_t* d_slot,
                       float* d_conf, float* d_value, const float* d_depth,
                       const double* d_tf, const double* d_values,
@@ -96,15 +98,18 @@ int vlfm_value_mask_unexplored(int G, int C, int batch, const int32_t* d_slot, f
 /* Replaces ValueMap.sort_waypoints' inner pixel_value_within_radius
  * (value_map.py:163-176, img_utils.py:213-266): median of the non-zero cells of
  * channel c inside the radius-`radius` disc (d_disc: (2r+1)^2 uint8 mask as drawn by
- * cv2.circle) around (row,col) = d_points[i]; -1 when empty.
+ * cv2.circle) around (row,col) = d_points[i]; -1 when empty.  radius 0..31.
+ * grid_f64: the dtype np.median would see -- 1 for weighted maps (the reference's value grid is
+ * float64 after the first fuse), 0 for max-confidence and replace maps (float32): the midpoint
+ * of an even count is computed in that precision.
  * d_out [npoints, C] float64.                                                       */
 int vlfm_value_disc_median(int G, int C, int slot, const float* d_value, const int32_t* d_points,
-                           int npoints, int radius, const uint8_t* d_disc, double* d_out,
+                           int npoints, int radius, int grid_f64, const uint8_t* d_disc, double* d_out,
                            void* stream);
 /* The same for the frontiers of MANY environments in one launch: d_points_srl [npoints,3] int32 = (slot, row, col),
  * d_value [nslots,G,G,C]; d_out [npoints,C].  (ITMPolicy._sort_frontiers_by_value, itm_policy.py:263-294, per env.) */
 int vlfm_value_disc_median_batch(int G, int C, const float* d_value, const int32_t* d_points_srl, int npoints, int radius,
-                                 const uint8_t* d_disc, double* d_out, void* stream);
+                                 int grid_f64, const uint8_t* d_disc, double* d_out, void* stream);
 
 /* --------------------------------------------------------------- obstacle map ---- */
 /* Replaces ObstacleMap.update_map obstacle half (vlfm/mapping/obstacle_map.py:86-109):
@@ -126,7 +131,8 @@ typedef struct VlfmObstacleParams {
 /* d_obst [nslots,G,G] uint8 (ObstacleMap._map), d_nav [nslots,G,G] uint8
  * (ObstacleMap._navigable_map as 0/1).                                               */
 /* d_hole_fill [batch,H,W] uint8 or NULL: output of vlfm_fill_small_holes (pixels whose depth becomes 1.0);
- * NULL selects the hole_area_thresh == -1 form (every zero depth becomes 1.0, obstacle_map.py:87-89). */
+ * NULL selects the hole_area_thresh == -1 form (every zero depth becomes 1.0, obstacle_map.py:87-89).
+ * d_status [batch] int32, indexed by call row. */
 int vlfm_obstacle_update(const VlfmObstacleParams* p, int batch, const int32_t* d_slot,
                          uint8_t* d_obst, uint8_t* d_nav, const float* d_depth,
                          const double* d_tf, const uint8_t* d_hole_fill, int32_t* d_status, void* stream);

@@ -61,8 +61,8 @@ _SIGNATURES = {
     "vlfm_value_workspace_bytes": (C.c_int, [C.POINTER(ValueParams), C.c_int, C.POINTER(C.c_size_t)]),
     "vlfm_value_update": (C.c_int, [C.POINTER(ValueParams), C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "vlfm_value_mask_unexplored": (C.c_int, [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
-    "vlfm_value_disc_median": (C.c_int, [C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
-    "vlfm_value_disc_median_batch": (C.c_int, [C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "vlfm_value_disc_median": (C.c_int, [C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "vlfm_value_disc_median_batch": (C.c_int, [C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "vlfm_obstacle_update": (C.c_int, [C.POINTER(ObstacleParams), C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "vlfm_value_cone_template": (C.c_int, [C.c_double, C.c_double, C.c_int, C.c_double, _P, _P, C.c_size_t, _P]),
     "vlfm_biattn_f16": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _P]),

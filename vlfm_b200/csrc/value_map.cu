@@ -120,7 +120,7 @@ __device__ __forceinline__ void edge_row(uint32_t* tog, uint32_t* orb, int WPR, 
 __global__ void __launch_bounds__(K1_THREADS)
 value_depth_geom_kernel(ValueDev p, const float* __restrict__ depth, const double* __restrict__ tf,
                         const double* __restrict__ tanv, uint32_t* __restrict__ ws,
-                        int* __restrict__ status) {
+                        const int* __restrict__ slot, int* __restrict__ status) {
   extern __shared__ __align__(16) uint32_t smem[];
   const int b = blockIdx.z;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -201,7 +201,7 @@ value_depth_geom_kernel(ValueDev p, const float* __restrict__ depth, const doubl
       int px = (int)__dmul_rn(cx, (double)p.ppm) + p.G / 2;
       int py = (int)__dmul_rn(-cy, (double)p.ppm) + p.G / 2;
       int valid = (px >= 0 && px < p.G && py >= 0 && py < p.G);
-      if (!valid) atomicOr(&status[b], VLFM_ST_CAMERA_OFF_GRID);
+      if (!valid) atomicOr(&status[slot ? slot[b] : b], VLFM_ST_CAMERA_OFF_GRID);   // flags belong to the grid slot
       wsb[p.offHeader + 0] = (uint32_t)px;
       wsb[p.offHeader + 1] = (uint32_t)py;
       wsb[p.offHeader + 2] = (uint32_t)valid;
@@ -477,10 +477,12 @@ __global__ void value_mask_unexplored_kernel(int G, int C, const int* __restrict
 
 // pixel_value_within_radius (img_utils.py:213-266), reduction="median".
 // one block per (point, channel); bitonic sort of the <= CAP candidate values (CAP = 1024: radius <= 15 cells, 4096: <= 31).
+// np.median averages the two middle values of an even count in the grid's dtype: float64 for the reference's weighted maps
+// (grid_f64 = 1), float32 for max-confidence and replace maps, whose value grid stays float32 (grid_f64 = 0).
 template <int CAP>
 __global__ void __launch_bounds__(256)
 value_disc_median_kernel(int G, int C, const float* __restrict__ valueAll, const int* __restrict__ pts, int with_slot,
-                         int radius, const uint8_t* __restrict__ disc, double* __restrict__ out) {
+                         int radius, int grid_f64, const uint8_t* __restrict__ disc, double* __restrict__ out) {
   __shared__ float vals[CAP];
   __shared__ int s_n;
   const int pi = blockIdx.x, ch = blockIdx.y, tid = threadIdx.x;
@@ -523,7 +525,8 @@ value_disc_median_kernel(int G, int C, const float* __restrict__ valueAll, const
     double r;
     if (n == 0) r = -1.0;
     else if (n & 1) r = (double)vals[n / 2];
-    else r = ((double)vals[n / 2 - 1] + (double)vals[n / 2]) * 0.5;
+    else if (grid_f64) r = ((double)vals[n / 2 - 1] + (double)vals[n / 2]) * 0.5;
+    else r = (double)__fmul_rn(__fadd_rn(vals[n / 2 - 1], vals[n / 2]), 0.5f);
     out[(size_t)pi * C + ch] = r;
   }
 }
@@ -571,7 +574,7 @@ extern "C" int vlfm_value_update(const VlfmValueParams* p, int batch, const int3
     if (rc) return rc; cfg2 = sm2;
   }
   dim3 g1(d.nColTiles, d.nChunks, batch);
-  value_depth_geom_kernel<<<g1, K1_THREADS, 8 * K1_COLS * 4, st>>>(d, d_depth, d_tf, d_tan, (uint32_t*)d_workspace, d_status);
+  value_depth_geom_kernel<<<g1, K1_THREADS, 8 * K1_COLS * 4, st>>>(d, d_depth, d_tf, d_tan, (uint32_t*)d_workspace, d_slot, d_status);
   VLFM_CHECK_LAUNCH("value_depth_geom_kernel");
   {
     int rc = check_cuda(launch_pdl(value_geom_kernel, dim3(batch), dim3(GEOM_THREADS), sm1, st, d, d_tan, (uint32_t*)d_workspace), "value_geom_kernel");
@@ -608,7 +611,7 @@ extern "C" int vlfm_value_mask_unexplored(int G, int C, int batch, const int32_t
 }
 
 extern "C" int vlfm_value_disc_median(int G, int C, int slot, const float* d_value, const int32_t* d_points,
-                                      int npoints, int radius, const uint8_t* d_disc, double* d_out,
+                                      int npoints, int radius, int grid_f64, const uint8_t* d_disc, double* d_out,
                                       void* stream) {
   if (!d_value || !d_points || !d_disc || !d_out || radius < 0 || radius > 31 || C < 1) {
     set_error("vlfm_value_disc_median: bad argument (radius must be <= 31 cells)"); return VLFM_E_INVALID; }
@@ -616,23 +619,23 @@ extern "C" int vlfm_value_disc_median(int G, int C, int slot, const float* d_val
   dim3 g(npoints, C);
   if (radius <= 15)
     value_disc_median_kernel<1024><<<g, 256, 0, (cudaStream_t)stream>>>(G, C, d_value + (size_t)slot * G * G * C,
-                                                                       d_points, 0, radius, d_disc, d_out);
+                                                                       d_points, 0, radius, grid_f64, d_disc, d_out);
   else
     value_disc_median_kernel<4096><<<g, 256, 0, (cudaStream_t)stream>>>(G, C, d_value + (size_t)slot * G * G * C,
-                                                                       d_points, 0, radius, d_disc, d_out);
+                                                                       d_points, 0, radius, grid_f64, d_disc, d_out);
   VLFM_CHECK_LAUNCH("value_disc_median_kernel");
   count_launch();
   return VLFM_OK;
 }
 
 extern "C" int vlfm_value_disc_median_batch(int G, int C, const float* d_value, const int32_t* d_points_srl, int npoints, int radius,
-                                            const uint8_t* d_disc, double* d_out, void* stream) {
+                                            int grid_f64, const uint8_t* d_disc, double* d_out, void* stream) {
   if (!d_value || !d_points_srl || !d_disc || !d_out || radius < 0 || radius > 31 || C < 1) {
     set_error("vlfm_value_disc_median_batch: bad argument (radius must be <= 31 cells)"); return VLFM_E_INVALID; }
   if (npoints <= 0) return VLFM_OK;
   dim3 g(npoints, C);
-  if (radius <= 15) value_disc_median_kernel<1024><<<g, 256, 0, (cudaStream_t)stream>>>(G, C, d_value, d_points_srl, 1, radius, d_disc, d_out);
-  else value_disc_median_kernel<4096><<<g, 256, 0, (cudaStream_t)stream>>>(G, C, d_value, d_points_srl, 1, radius, d_disc, d_out);
+  if (radius <= 15) value_disc_median_kernel<1024><<<g, 256, 0, (cudaStream_t)stream>>>(G, C, d_value, d_points_srl, 1, radius, grid_f64, d_disc, d_out);
+  else value_disc_median_kernel<4096><<<g, 256, 0, (cudaStream_t)stream>>>(G, C, d_value, d_points_srl, 1, radius, grid_f64, d_disc, d_out);
   VLFM_CHECK_LAUNCH("value_disc_median_kernel");
   count_launch();
   return VLFM_OK;

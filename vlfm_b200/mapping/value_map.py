@@ -99,7 +99,7 @@ class ValueMapBatch:
         self.fusion = fusion_code(use_max_confidence, fusion_type)
         self.conf = torch.zeros((batch, size, size), dtype=torch.float32, device=self.device)
         self.value = torch.zeros((batch, size, size, value_channels), dtype=torch.float32, device=self.device)
-        self.status = torch.zeros((batch,), dtype=torch.int32, device=self.device)
+        self.status = torch.zeros((batch,), dtype=torch.int32, device=self.device)   # VLFM_ST_* flags per grid SLOT, like conf / value
         self._ws: Optional[torch.Tensor] = None
         self._ws_key: Optional[Tuple[int, int, int]] = None
         self.rows_per_tile = 0
@@ -155,12 +155,13 @@ class ValueMapBatch:
         _lib.check(rc, "vlfm_value_mask_unexplored")
 
     def disc_median(self, slot: int, points_rc: np.ndarray, radius: int) -> np.ndarray:
-        """[(row, col)] -> [npoints, C] medians of non-zero cells in the disc (-1 if none)."""
+        """[(row, col)] -> [npoints, C] medians of non-zero cells in the disc (-1 if none), as np.median computes them on the
+        reference's grid: an even count's midpoint in float64 for weighted maps, in float32 otherwise (``ref_float64``)."""
         pts = torch.from_numpy(np.ascontiguousarray(points_rc, dtype=np.int32)).to(self.device)
         out = torch.empty((len(points_rc), self.channels), dtype=torch.float64, device=self.device)
         with torch.cuda.device(self.device):
             rc = self.lib.vlfm_value_disc_median(self.size, self.channels, slot, _lib.ptr(self.value), _lib.ptr(pts),
-                                                 len(points_rc), radius, _lib.ptr(_disc(radius, self.device)),
+                                                 len(points_rc), radius, int(self.ref_float64), _lib.ptr(_disc(radius, self.device)),
                                                  _lib.ptr(out), _lib.stream_ptr())
         _lib.check(rc, "vlfm_value_disc_median")
         return out.cpu().numpy()
@@ -173,7 +174,8 @@ class ValueMapBatch:
         out = torch.empty((len(points_srl), self.channels), dtype=torch.float64, device=self.device)
         with torch.cuda.device(self.device):
             rc = self.lib.vlfm_value_disc_median_batch(self.size, self.channels, _lib.ptr(self.value), _lib.ptr(pts), len(points_srl), radius,
-                                                       _lib.ptr(_disc(radius, self.device)), _lib.ptr(out), _lib.stream_ptr())
+                                                       int(self.ref_float64), _lib.ptr(_disc(radius, self.device)), _lib.ptr(out),
+                                                       _lib.stream_ptr())
         _lib.check(rc, "vlfm_value_disc_median_batch")
         return out.cpu().numpy()
 
@@ -201,6 +203,55 @@ class ValueMapBatch:
             self.conf.zero_(); self.value.zero_(); self.status.zero_()
         else:
             self.conf[slot].zero_(); self.value[slot].zero_(); self.status[slot] = 0
+
+    def waypoint_values(self, med: np.ndarray, reduce_fn: Optional[Callable]) -> List[Any]:
+        """[npoints, C] disc medians -> the values the reference's sort_waypoints sorts (value_map.py:171-187): np.median's scalar
+        type (float64 for weighted maps, float32 otherwise) or the int -1 of an empty disc, one per point when C == 1, else
+        ``reduce_fn`` of the per-channel tuples.  The type matters: np.argsort is not stable, and the tie order it produces
+        depends on the dtype of the array it sorts."""
+        typ = np.float64 if self.ref_float64 else np.float32
+        if self.channels == 1:
+            return [typ(m[0]) if m[0] != -1 else -1 for m in med]
+        assert reduce_fn is not None, "Must provide a reduction function when using multiple value channels."
+        return reduce_fn([tuple(typ(v) if v != -1 else -1 for v in m) for m in med])
+
+
+def frontier_values(omb: Any, vmb: ValueMapBatch, n: int, radius_m: float, reduce_fn: Optional[Callable] = None
+                    ) -> List[Tuple[np.ndarray, List[Any]]]:
+    """ITMPolicy._sort_frontiers_by_value (itm_policy.py:263-266) for slots 0..n-1 of an ObstacleMapBatch ``omb`` and a ValueMapBatch
+    ``vmb``: each environment's frontiers in metres (ObstacleMap.frontiers) sorted and scored exactly as
+    ``ValueMap.sort_waypoints(frontiers, radius_m)`` does it -- metres to cells with int() truncation (value_map.py:163-170), the
+    disc median of every frontier of every environment in one launch and one read-back, np.argsort of the negated values.
+    Returns [(frontiers [F, 2] sorted, values)] per environment.
+
+    A zero-length frontier piece has a NaN midpoint (its arc-length midpoint is 0/0).  The reference's int(NaN) raises ValueError
+    there, which would end the step of every environment in the batch; here such a frontier gets the value -1, the value of a
+    frontier with no observed cell in its disc, and so sorts behind every frontier that has a value.  A finite point off the grid
+    raises AssertionError, as pixel_value_within_radius does (img_utils.py:43)."""
+    g, ppm = vmb.size, vmb.ppm
+    assert omb.size == g and omb.ppm == ppm
+    fronts = omb.all_frontiers_px(n)
+    counts = [len(px) for px in fronts]
+    out: List[Tuple[np.ndarray, List[Any]]] = [(np.array([]), []) for _ in range(n)]
+    if sum(counts) == 0:
+        return out
+    xy = omb.px_to_xy(np.concatenate([px for px in fronts if len(px)]))      # every environment's frontiers, in metres
+    env = np.repeat(np.arange(n), counts)
+    ok = ~np.isnan(xy).any(axis=1)
+    row = g - (np.trunc(-xy[ok, 0] * ppm) + g // 2)          # size - (int(-x * ppm) + origin[0])
+    col = np.trunc(-xy[ok, 1] * ppm) + g // 2                # int(-y * ppm) + origin[1]
+    assert ((row >= 0) & (row < g) & (col >= 0) & (col < g)).all(), "Pixel location is outside the image."
+    med = np.full((len(xy), vmb.channels), -1.0)
+    if ok.any():
+        med[ok] = vmb.disc_median_batch(np.stack([env[ok], row, col], axis=1).astype(np.int64), int(radius_m * ppm))
+    k = 0
+    for e, c in enumerate(counts):
+        if c:
+            values = vmb.waypoint_values(med[k:k + c], reduce_fn)
+            order = np.argsort([-v for v in values])
+            out[e] = (xy[k:k + c][order], [values[i] for i in order])
+        k += c
+    return out
 
 
 class ValueMap(BaseMap):
@@ -324,11 +375,7 @@ class ValueMap(BaseMap):
         if len(pts) == 0:
             return np.array([]), []
         med = self._eng.disc_median(0, np.array(pts), radius_px)
-        if self._value_channels == 1:
-            values: List[Any] = [float(m[0]) if m[0] != -1 else -1 for m in med]
-        else:
-            assert reduce_fn is not None, "Must provide a reduction function when using multiple value channels."
-            values = reduce_fn([tuple(float(v) if v != -1 else -1 for v in m) for m in med])
+        values = self._eng.waypoint_values(med, reduce_fn)
         order = np.argsort([-v for v in values])
         return np.array([waypoints[i] for i in order]), [values[i] for i in order]
 

@@ -12,6 +12,8 @@ from typing import Any, Dict, List, Optional
 import numpy as np
 import torch
 
+from ..mapping.value_map import frontier_values
+
 MIN_D, MAX_D, FOV = 0.5, 5.0, float(np.deg2rad(79))
 PROMPT = "Seems like there is a chair ahead."
 CAPTION = "chair . couch . potted plant . bed . toilet . tv ."
@@ -117,17 +119,8 @@ class FullStep:
 
         def score():
             # ITMPolicy._sort_frontiers_by_value for every environment: one D2H of the frontier lists, one disc-median launch, one D2H
-            fronts = self.omb.all_frontiers_px(B)
-            pts = []
-            for e, px in enumerate(fronts):
-                self.n_front += len(px)
-                if len(px):
-                    xy = self.omb.px_to_xy(px)                     # ObstacleMap.frontiers (metres) ...
-                    with np.errstate(invalid="ignore"):             # a zero-length frontier piece has a NaN midpoint (0/0), as in the reference
-                        q = self.omb.xy_to_px(xy[:, :2])            # ... and back to cells, as the policy does through sort_waypoints
-                    pts.append(np.stack([np.full(len(q), e), q[:, 1], q[:, 0]], axis=1))
-            if pts:
-                self.vmb.disc_median_batch(np.concatenate(pts), int(0.5 * self.ppm))
+            for fr, _ in frontier_values(self.omb, self.vmb, B, 0.5):
+                self.n_front += len(fr)
 
         on(main, "frontier_scoring", score)
         if conc:
