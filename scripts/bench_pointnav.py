@@ -87,7 +87,6 @@ def main() -> None:
         masks = torch.ones(B, dtype=torch.bool, device="cuda")
         ids = torch.arange(B, device="cuda")
         eng = pol.engine
-        eng.step(frames, goal, masks, ids)     # eager + capture
         hidden = torch.zeros(B, 4, 512, device="cuda")
         prev = torch.zeros(B, 1, dtype=torch.long, device="cuda")
         with torch.inference_mode():

@@ -51,7 +51,7 @@ def main():
         imgs = torch.from_numpy(rng.integers(0, 256, (B, 480, 640, 3), dtype=np.uint8)).cuda()
         e.run(imgs)
         e.run(imgs)
-        g, _ = e._graphs[(B, 480, 640)]
+        g = e.graphs.captured[(B, 480, 640)].graph
         x = O.preprocess(imgs[0].cpu().numpy()).cuda().half().repeat(B, 1, 1, 1)
         fp16 = lambda: O.forward(e.layers, x, dtype=torch.float16)
         with torch.inference_mode():
@@ -68,7 +68,7 @@ def main():
     # split of one batch-1 replay by kernel name (profiler run of its own)
     from torch.profiler import ProfilerActivity, profile
 
-    g, _ = e._graphs[(1, 480, 640)]
+    g = e.graphs.captured[(1, 480, 640)].graph
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for _ in range(5):
             g.replay()

@@ -37,4 +37,4 @@ for i in range(a.steps):
     if i == a.profile_step:
         torch.cuda.profiler.stop()
     fr = om._frame(0)
-    print(f"step {i}: {ev[0].elapsed_time(ev[1])*1e3:.0f} us  graph={'yes' if om._graphs else 'no'}  S frame env0 {fr[2]-fr[0]}x{fr[3]-fr[1]}  frontiers {om.count[:B].tolist()[:6]}  status {int(om.ex_status.max())}", flush=True)
+    print(f"step {i}: {ev[0].elapsed_time(ev[1])*1e3:.0f} us  graph={'yes' if om.graphs.captured else 'no'}  S frame env0 {fr[2]-fr[0]}x{fr[3]-fr[1]}  frontiers {om.count[:B].tolist()[:6]}  status {int(om.ex_status.max())}", flush=True)

@@ -23,7 +23,7 @@ def hook(name):
         e = torch.cuda.Event(enable_timing=True); e.record(); times[name][-1][1] = e
     return pre, post
 # GdinoForward sequences the encoder / decoder stacks itself: the per-layer modules are what is called.  Hooks fire on eager
-# forwards only (B above VLFM_GDINO_GRAPH_MAX_BATCH, or VLFM_GDINO_GRAPH=0).
+# forwards only (B above GRAPH_MAX_BATCH, or VLFM_NO_GRAPH=1).
 mods = []
 for l in gd.model.model.encoder.layers:
     mods += [("enc.fusion", l.fusion_layer), ("enc.text_enh", l.text_enhancer_layer), ("enc.deform", l.deformable_layer)]

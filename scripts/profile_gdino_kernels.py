@@ -1,7 +1,7 @@
 """One eager GroundingDINO forward (batch from $B) between cudaProfilerStart/Stop, for ncu kernel filters."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-os.environ["VLFM_GDINO_GRAPH"] = "0"
+os.environ["VLFM_NO_GRAPH"] = "1"
 import numpy as np, torch
 from vlfm_b200.vlm.grounding_dino import GroundingDINO
 B = int(os.environ.get("B", "8"))

@@ -2,7 +2,7 @@
 one-pass trace, warp-parallel rays), value K2, x2 GEMM / fp32 attention / LayerNorm x2 (TINY BLIP-2 forward), radix-select top-k, object cloud."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-os.environ.setdefault("VLFM_MAP_GRAPH", "0")
+os.environ.setdefault("VLFM_NO_GRAPH", "1")
 import numpy as np, torch
 from vlfm_b200.mapping.obstacle_batch import ObstacleMapBatch
 from vlfm_b200.mapping.value_map import ValueMapBatch

@@ -107,10 +107,12 @@ def test_rows_independent_bitwise(full, B):
 def test_graph_replays_and_eager_bitwise(full, B):
     """three graph replays on distinct copies of one batch agree to the bit, and so does the eager (uncaptured) forward"""
     m, Q = full.m, full.dims.queries
+    m.cosine_device_many(full.dev[:B].clone(), PROMPTS)          # warm-up: the first call of a shape runs eagerly
     outs = []
     for _ in range(3):
         c = m.cosine_device_many(full.dev[:B].clone(), PROMPTS).clone()
         outs.append((c, m.engine.q_proj[: B * Q].clone()))
+    assert (B, *full.dev.shape[1:3]) in m.engine.graphs.captured
     m.engine.use_graph = False
     try:
         c = m.cosine_device_many(full.dev[:B].clone(), PROMPTS).clone()

@@ -19,7 +19,8 @@ def test_preprocess_matches_pil_bit_exact():
     from vlfm_b200.vlm.blip2_engine import Blip2ITCEngine
 
     d = SMALL
-    eng = Blip2ITCEngine(d, random_state_dict(d, 0), max_batch=2, use_graph=False)
+    eng = Blip2ITCEngine(d, random_state_dict(d, 0), max_batch=2)
+    eng.use_graph = False
     rng = np.random.default_rng(0)
     imgs = np.stack([make_rgb(rng, 480, 640), make_rgb(rng, 480, 640)])
     dev = torch.from_numpy(imgs).cuda()

@@ -425,30 +425,32 @@ def test_detector_batches_match_single_frames(biased):
     ids = det.tokenizer.encode("chair . couch . tv .")
     rng = np.random.default_rng(31)
     imgs = np.stack([make_rgb(rng, 480, 640) for _ in range(5)])
-    graph_ok = det._graph_ok
+    use_graph = det.use_graph
     try:
-        det._graph_ok = False
+        det.use_graph = False
         e0 = [t.clone() for t in det.raw_outputs(imgs[0], ids)]
         e1 = [t.clone() for t in det.raw_outputs(imgs[0], ids)]
     finally:
-        det._graph_ok = graph_ok
+        det.use_graph = use_graph
     ee = _detection_metrics(e0[0], e0[1], e1[0], e1[1])
     bar = (max(5e-3, 3 * ee[0]), max(1e-3, 3 * ee[1]))
     # back to back, as a policy loop calls it: the graph replays are enqueued faster than they run, so each call must keep
     # its own frame even though the next call refills the same page-locked staging buffer
     single = [[t.clone() for t in det.raw_outputs(img, ids)] for img in imgs]
-    assert det._graph_max_batch == 4
+    from vlfm_b200.vlm.grounding_dino import GRAPH_MAX_BATCH
+
+    assert GRAPH_MAX_BATCH == 4
     other = _detection_metrics(single[0][0], single[0][1], single[1][0], single[1][1])
     res = []
     for b in (2, 5):
         d_imgs = torch.from_numpy(imgs[:b]).cuda()
         det.raw_outputs_device(d_imgs, ids)
         lg, bx = (t.clone() for t in det.raw_outputs_device(d_imgs, ids))
-        graph = det._static[(b, 480, 640, tuple(ids))]["graph"]
-        assert (graph is not None) == (b <= 4) and det.graph_error is None, det.graph_error
+        graph = (b, 480, 640, tuple(ids)) in det.graphs.captured
+        assert graph == (b <= 4) and det.graphs.error is None, det.graphs.error
         for i in range(b):
             res.append(_detection_metrics(single[i][0], single[i][1], lg[i], bx[i]))
-            print(f"B={b} ({'graph' if graph is not None else 'eager'}) image {i}: (confidence, box-set) {res[-1]}; eager vs eager {ee}; "
+            print(f"B={b} ({'graph' if graph else 'eager'}) image {i}: (confidence, box-set) {res[-1]}; eager vs eager {ee}; "
                   f"two different frames {other}")
     for m in res:
         assert m[0] <= bar[0] and m[1] <= bar[1]

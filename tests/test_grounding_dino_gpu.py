@@ -243,13 +243,13 @@ def test_batch1_cuda_graph_replay_matches_eager(pair):
         dist = (bb[:, None, :] - ba[None, :, :]).abs().sum(-1).min(dim=1)[0]
         return float((ca - cb).abs().mean()), float(dist.mean())
 
-    g._graph_ok = False                                               # eager baseline: same image twice
+    g.use_graph = False                                               # eager baseline: same image twice
     e0 = [t.clone() for t in g.raw_outputs(img1, ids)]
     e1 = [t.clone() for t in g.raw_outputs(img1, ids)]
-    g._graph_ok = True
+    g.use_graph = True
     g.raw_outputs(img2, ids)                                          # capture + first replay (this key already ran eagerly)
-    assert g.graph_error is None, g.graph_error
-    assert g._static[(1, 480, 640, tuple(ids))]["graph"] is not None
+    assert g.graphs.error is None, g.graphs.error
+    assert (1, 480, 640, tuple(ids)) in g.graphs.captured
     r = [t.clone() for t in g.raw_outputs(img1, ids)]                 # replay
     ee, ge = metrics(e0[0], e0[1], e1[0], e1[1]), metrics(e0[0], e0[1], r[0], r[1])
     print("eager vs eager (confidence, box-set):", ee, " graph vs eager:", ge)
@@ -292,7 +292,7 @@ def test_detection_decisions_match_the_fp32_twin(pair_calibrated):
     EPS16 = 2.0 ** -11
     cap = {}
     h1 = orc.model.model.decoder.register_forward_hook(lambda m_, a_, kw, o_: cap.__setitem__("ref", kw["reference_points"][0].detach().float().cpu()), with_kwargs=True)
-    graph_ok, g._graph_ok = g._graph_ok, False                                  # eager: every call sets g.fwd.last_reference_points
+    use_graph, g.use_graph = g.use_graph, False                                 # eager: every call sets g.fwd.last_reference_points
     stats = {"ours": [0, 0, 0, [], []], "twin": [0, 0, 0, [], []]}              # paired, unpaired, flipped, |dscore|, box L1
     try:
         for seed, caption in ((21, "chair . person . dog ."), (22, "couch . potted plant . tv .")):
@@ -327,7 +327,7 @@ def test_detection_decisions_match_the_fp32_twin(pair_calibrated):
                     st[3].append(abs(float(ref_l[i].max()) - float(dl[k].max())))
                     st[4].append(float((ref_b[i] - db[k]).abs().sum()))
     finally:
-        h1.remove(); g._graph_ok = graph_ok
+        h1.remove(); g.use_graph = use_graph
     rep = {}
     for name, st in stats.items():
         rep[name] = {"paired": st[0], "unpaired": st[1], "flipped": st[2] / max(st[0], 1), "dscore": float(np.mean(st[3])), "dbox": float(np.mean(st[4]))}

@@ -96,4 +96,4 @@ def test_graph_replay_with_static_buffers():
         eng.update(depth, tfs, tfd, 0.5, 5.0, fx, fx, FOV)
         for e in range(B):
             _check(eng, e, orc[e], f"step {i} env {e}")
-    assert eng.use_graph and len(eng._graphs) == 1, "the update was never captured"
+    assert eng.use_graph and len(eng.graphs.captured) == 1, "the update was never captured"

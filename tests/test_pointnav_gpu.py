@@ -96,11 +96,13 @@ def test_graph_replay_equals_eager_and_repeats():
     runs = []
     for graph in (True, False, True):
         pol = PointNavBatch(sd, max_batch=B)
+        pol.engine.use_graph = graph
         outs = []
         for t in range(4):
             pol.engine.step(torch.from_numpy(frames[t]).cuda(), torch.from_numpy(goals[t]).cuda(), torch.from_numpy(masks[t]).cuda(),
-                            torch.arange(B).cuda(), graph=graph)
+                            torch.arange(B).cuda())
             outs.append((pol.engine.head[:B].clone(), pol.hidden_states.clone(), pol.engine.action[:B].clone()))
+        assert ((B, 224, 224) in pol.engine.graphs.captured) == graph
         runs.append(outs)
     for a, b in zip(runs[0], runs[1]):
         for x, y in zip(a, b):

@@ -166,10 +166,15 @@ def test_predict_device_batches_match_single_frames(model):
 def test_graph_replay_equals_eager_and_repeats(model):
     img = torch.from_numpy(np.stack([frame((720, 1280), 3), frame((720, 1280), 4)])).cuda()
     e = model.engine
-    eager = [t.clone() for t in e.run(img, graph=False)]
+    e.use_graph = False
+    try:
+        eager = [t.clone() for t in e.run(img)]
+    finally:
+        e.use_graph = True
     heads_eager = [t.clone() for t in e._bufs[2]["head"]]
     for _ in range(3):
-        got = e.run(img, graph=True)
+        got = e.run(img)
+        assert (2, 720, 1280) in e.graphs.captured
         for a, b in zip(got, eager):
             assert torch.equal(a.view(torch.int32) if a.is_floating_point() else a, b.view(torch.int32) if b.is_floating_point() else b)
         for a, b in zip(e._bufs[2]["head"], heads_eager):
@@ -196,12 +201,13 @@ def test_predict_and_client_surface(model, monkeypatch):
     det2.filter_by_conf(0.3)
     assert torch.all(det2.logits >= 0.3)
     # thresholds and classes change without re-capturing
-    ngraph = len(model.engine._graphs)
+    assert (1, 480, 640) in model.engine.graphs.captured
+    ngraph = len(model.engine.graphs.captured)
     strict = model.predict(img, conf_thres=0.6)
     assert strict.num_detections <= det.num_detections and torch.all(strict.logits > 0.6)
     only = model.predict(img, classes=[56, 57])
     assert set(only.phrases) <= {"chair", "couch"}
-    assert len(model.engine._graphs) == ngraph
+    assert len(model.engine.graphs.captured) == ngraph
     monkeypatch.setenv("VLFM_SYNTHETIC_WEIGHTS", "1")
     monkeypatch.setattr(Y, "_SHARED", {"default": model})
     assert Y.YOLOv7Client().model is model

@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from .. import _lib
+from ..utils.cuda_graph import GraphCache, default_use_graph
 from . import render as _render
 from . import sframe as _sf
 
@@ -71,14 +72,10 @@ class ObstacleMapBatch:
         self._fill_status = torch.zeros((batch,), dtype=torch.int32, device=dev)
         self._slot_ids = torch.arange(batch, dtype=torch.int32, device=dev)
         # CUDA graph of the whole update (hole fill + scatter + dilate + explore): the launch geometry of every C-ABI call depends on
-        # the batch size only and the per-environment pose scalars travel in page-locked records, so after two eager calls with the
-        # same buffers the sequence is captured once and replayed (VLFM_MAP_GRAPH=0 disables; ~75 launches -> one graph launch)
-        import os
-
-        self.use_graph = os.environ.get("VLFM_MAP_GRAPH", "1") != "0"
-        self._graphs = {}
-        self._graph_key = None
-        self._graph_seen = 0
+        # the batch size only and the per-environment pose scalars travel in page-locked records, so the second call with the same
+        # buffers and parameters captures the sequence and later ones replay it (~75 launches -> one graph launch)
+        self.use_graph = default_use_graph()
+        self.graphs = GraphCache(max_keys=4)
         self._rec_pin = torch.zeros(rec * batch, dtype=torch.uint8).pin_memory()      # explore records read by the captured upload node
         self._rec_ev = torch.cuda.Event()
         self._rec_used = False
@@ -128,19 +125,19 @@ class ObstacleMapBatch:
             e.max_line_len = float(max_depth * ppm)
             e.area_thresh_px = float(self.area_thresh_px)
 
-    def _device_sequence(self, n: int, depth, tf_dev, p, slot_t, explore: bool, update_obstacles: bool, rec_pin: Optional[torch.Tensor]) -> None:
-        """the launches of one update on the current stream (eager or under CUDA-graph capture)"""
+    def _device_sequence(self, n: int, depth, tf_dev, p, slot_t, explore: bool, update_obstacles: bool, pins: Optional[Tuple[torch.Tensor, ...]]) -> None:
+        """the launches of one update on the current stream: eager, or for a graph with ``pins`` = its (explore, hole-fill) record buffers"""
         st = _lib.stream_ptr()
         g = self.size
         if update_obstacles:
             h, w = int(depth.shape[1]), int(depth.shape[2])
             fill = None
             if self.hole_area_thresh != -1:          # fill_small_holes (img_utils.py:361-390) on the device
-                pin = self._pinned() if rec_pin is None else self._holes_pin
+                pin = self._pinned() if pins is None else pins[1]
                 rc = self.lib.vlfm_fill_small_holes_batch(_lib.ptr(depth), h, w, n, float(self.hole_area_thresh), _lib.ptr(self._fill),
                                                           _lib.ptr(self._fill_ws), self._fill_ws.numel() * 4, _lib.ptr(self._fill_status),
                                                           pin.data_ptr(), pin.numel(), st)
-                if rec_pin is None:
+                if pins is None:
                     self._pinned_done()
                 _lib.check(rc, "vlfm_fill_small_holes_batch")
                 fill = self._fill
@@ -149,15 +146,15 @@ class ObstacleMapBatch:
             _lib.check(rc, "vlfm_obstacle_update")
         if not explore:
             return
-        if rec_pin is None:
+        if pins is None:
             pin = self._pinned()
             rc = self.lib.vlfm_explore_update_batch(g, n, self._envs, _lib.ptr(self.explored), _lib.ptr(self.nav), _lib.ptr(self._call_front),
                                                     _lib.ptr(self._call_count), _lib.ptr(self._call_status), _lib.ptr(self._ex_ws),
                                                     self._ex_ws.numel() * 4, pin.data_ptr(), pin.numel(), st)
             self._pinned_done()
             _lib.check(rc, "vlfm_explore_update_batch")
-        else:                                        # records already prepared in rec_pin by the caller
-            _lib.check(self.lib.vlfm_explore_launch_batch(g, n, _lib.ptr(self._ex_ws), rec_pin.data_ptr(), st), "vlfm_explore_launch_batch")
+        else:                                        # records already prepared in pins[0] by the caller
+            _lib.check(self.lib.vlfm_explore_launch_batch(g, n, _lib.ptr(self._ex_ws), pins[0].data_ptr(), st), "vlfm_explore_launch_batch")
         if slot_t is None:
             self.frontiers[:n].copy_(self._call_front[:n]); self.count[:n].copy_(self._call_count[:n]); self.ex_status[:n].copy_(self._call_status[:n])
         else:
@@ -193,43 +190,33 @@ class ObstacleMapBatch:
                     _lib.check(self.lib.vlfm_holes_batch_workspace_bytes(h, w, self.batch, ctypes.byref(nb)), "vlfm_holes_batch_workspace_bytes")
                     self._fill = torch.zeros((self.batch, h, w), dtype=torch.uint8, device=self.device)
                     self._fill_ws = torch.zeros((nb.value + 3) // 4, dtype=torch.int32, device=self.device)
-                    self._holes_pin = torch.zeros(self._pin[0].numel(), dtype=torch.uint8).pin_memory()
-                    self._graphs.clear()
+                    self.graphs.clear()
                 for i, s in enumerate(slots):
                     self._cover_add(s, _sf.obstacle_window(int(agents[i][0]), int(agents[i][1]), half, g))
                     self.nav_valid[s] = True
                 self._last_half = half
             if explore:
                 self._fill_envs(n, slots, agents, tf_host, max_depth, topdown_fov)
-            # ---- graph replay when the same buffers and parameters come back (the steady state of an episode loop)
-            key = None
-            if self.use_graph and identity and explore and update_obstacles and not first:
-                key = (n, depth.data_ptr(), tf_dev.data_ptr(), tuple(depth.shape), float(min_depth), float(max_depth), float(fx), float(fy), float(topdown_fov))
-            if key is not None and key == self._graph_key:
-                self._graph_seen += 1
-            else:
-                self._graph_key, self._graph_seen = key, 0
-            if key is not None and (key in self._graphs or self._graph_seen >= 1):
+            if not (identity and explore and update_obstacles and not first):
+                self._device_sequence(n, depth, tf_dev, p, slot_t, explore, update_obstacles, None)
+                return
+            key = (n, depth.data_ptr(), tf_dev.data_ptr(), tuple(depth.shape), float(min_depth), float(max_depth), float(fx), float(fy), float(topdown_fov))
+            pins = None
+            if self.graphs.will_replay(key, self.use_graph):
                 if self._rec_used:
                     self._rec_ev.synchronize()           # the previous replay's record upload has executed
                 rc = self.lib.vlfm_explore_prepare_batch(g, n, self._envs, _lib.ptr(self.explored), _lib.ptr(self.nav), _lib.ptr(self._call_front),
                                                          _lib.ptr(self._call_count), _lib.ptr(self._call_status), _lib.ptr(self._ex_ws),
                                                          self._ex_ws.numel() * 4, self._rec_pin.data_ptr(), self._rec_pin.numel())
                 _lib.check(rc, "vlfm_explore_prepare_batch")
-                gr = self._graphs.get(key)
-                if gr is None:
-                    torch.cuda.synchronize()
-                    gr = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(gr):
-                        self._device_sequence(n, depth, tf_dev, p, None, True, True, self._rec_pin)
-                    if len(self._graphs) >= 4:
-                        self._graphs.pop(next(iter(self._graphs)))
-                    self._graphs[key] = gr
-                gr.replay()
+                # a graph uploads its hole-fill records, which hold its depth pointer, from a page-locked buffer of its own: the
+                # capturing call allocates it and returns it, so it lives as long as the graph
+                holes = None if key in self.graphs.captured else torch.zeros(self._pin[0].numel(), dtype=torch.uint8).pin_memory()
+                pins = (self._rec_pin, holes)
+            self.graphs(key, self.use_graph, lambda: (self._device_sequence(n, depth, tf_dev, p, None, True, True, pins), pins))
+            if pins is not None:
                 self._rec_ev.record()
                 self._rec_used = True
-                return
-            self._device_sequence(n, depth, tf_dev, p, slot_t, explore, update_obstacles, None)
 
     # ----------------------------------------------------------------- readback ----
     def check_fill(self, slot: int = 0) -> None:

@@ -8,18 +8,18 @@ GEMM output.  Recurrent part in fp32: ``visual_fc`` (weight columns permuted
 from the NCHW flatten to NHWC), the two LSTM gate GEMMs ([x | h] @ [W_ih | W_hh]^T + b_ih + b_hh) on
 ``vlfm_pointnav_gemv_f32``, the cells and the head on ``vlfm_pointnav_lstm_*``.
 
-The step for a batch size and frame size is captured in a CUDA graph on its first call and replayed after; every launch is
-deterministic, so a replay is bitwise equal to an eager run.  An environment's result does not depend on the batch it shares,
-except through the conv GEMMs, whose row tiling depends on the batch size.
+The step for a batch size and frame size is captured in a CUDA graph on its second call and replayed after
+(``utils/cuda_graph.py``); every launch is deterministic, so a replay is bitwise equal to an eager run.  An environment's
+result does not depend on the batch it shares, except through the conv GEMMs, whose row tiling depends on the batch size.
 """
 from __future__ import annotations
 
-import os
 from typing import Dict, List, Optional, Tuple
 
 import torch
 
 from .. import _lib
+from ..utils.cuda_graph import GraphCache, default_use_graph
 from ..vlm.dense import conv_rows, gemm_f16, im2col
 from .pointnav_weights import BACKBONE, EMB, HEAD_CONTINUOUS, HEAD_DISCRETE, HID, NGROUPS, STAGES, VIS
 
@@ -54,7 +54,7 @@ def spatial_plan(hw: Tuple[int, int]) -> List[Tuple[int, int]]:
 
 class PointNavEngine:
     def __init__(self, w: Dict[str, torch.Tensor], discrete: bool, max_batch: int = 1, input_hw: Tuple[int, int] = (224, 224),
-                 num_envs: Optional[int] = None, device="cuda", use_graph: bool = True) -> None:
+                 num_envs: Optional[int] = None, device="cuda") -> None:
         if not torch.cuda.is_available():
             raise _lib.VlfmError("vlfm_b200 needs a CUDA device (no CPU fallback)")
         if not 1 <= max_batch <= MAX_GEMV_BATCH:
@@ -64,7 +64,7 @@ class PointNavEngine:
         self.discrete, self.max_batch, self.input_hw = discrete, max_batch, tuple(input_hw)
         self.num_envs = num_envs or max_batch
         self.sizes = spatial_plan(self.input_hw)
-        self.use_graph = use_graph and os.environ.get("VLFM_NO_GRAPH", "") != "1"
+        self.use_graph = default_use_graph()
         dev = self.dev
         f = lambda t: t.to(dev, F32).contiguous()
         self.w: Dict[str, torch.Tensor] = {}
@@ -117,7 +117,7 @@ class PointNavEngine:
         self.x16 = torch.empty(act, dtype=F16, device=dev)
         self.t16 = torch.empty(act, dtype=F16, device=dev)
         self.g16 = torch.empty(act, dtype=F16, device=dev)
-        self._graphs: Dict[Tuple[int, int, int], Tuple[torch.cuda.CUDAGraph, torch.Tensor]] = {}
+        self.graphs = GraphCache()   # no bound: every batch size is a key of its own
 
     # ---------------------------------------------------------------------------------------------------------- launches
     def _gemm(self, a_buf, M, K, wname, out_buf, N):
@@ -197,31 +197,15 @@ class PointNavEngine:
 
     # ------------------------------------------------------------------------------------------------------------- step
     @torch.inference_mode()
-    def step(self, depth: torch.Tensor, goal: torch.Tensor, masks: torch.Tensor, env_ids: torch.Tensor, graph: Optional[bool] = None) -> None:
+    def step(self, depth: torch.Tensor, goal: torch.Tensor, masks: torch.Tensor, env_ids: torch.Tensor) -> None:
         """depth [B,H,W] fp32 (device, any frame size), goal [B,2], masks [B] bool, env_ids [B] int (distinct state slots).  Writes
-        self.action / head / features [:B] and updates self.hidden / self.prev at env_ids.  ``graph=False`` runs eagerly."""
+        self.action / head / features [:B] and updates self.hidden / self.prev at env_ids."""
         B = depth.shape[0]
-        key = (B, depth.shape[1], depth.shape[2])
         with torch.cuda.device(self.dev):
             self.goal[:B].copy_(goal, non_blocking=True)
             self.masks[:B].copy_(masks, non_blocking=True)
             self.env_ids[:B].copy_(env_ids, non_blocking=True)
-            use_graph = self.use_graph if graph is None else graph
-            if not use_graph:
-                self._forward(depth.contiguous())
-                return
-            if key not in self._graphs:
-                static_in = depth.contiguous().clone()
-                self._forward(static_in)          # this call's step, eagerly; it also sets the kernels' attributes
-                torch.cuda.synchronize()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):          # capture records the launches without running them
-                    self._forward(static_in)
-                self._graphs[key] = (g, static_in)
-                return
-            g, static_in = self._graphs[key]
-            static_in.copy_(depth, non_blocking=True)
-            g.replay()
+            self.graphs((B, depth.shape[1], depth.shape[2]), self.use_graph, self._forward, depth.contiguous())
 
     def launches_per_step(self, B: int = 1, hw: Optional[Tuple[int, int]] = None) -> int:
         """Kernels one step launches (counted on an eager run that leaves the state unchanged)."""
@@ -229,9 +213,11 @@ class PointNavEngine:
         saved = (self.hidden.clone(), self.prev.clone())
         depth = torch.zeros(B, *hw, dtype=F32, device=self.dev)
         zeros = torch.zeros(B, dtype=torch.bool, device=self.dev)
+        use_graph, self.use_graph = self.use_graph, False
         n0 = _lib.launch_count()
-        self.step(depth, torch.zeros(B, 2, device=self.dev), zeros, torch.arange(B, device=self.dev), graph=False)
+        self.step(depth, torch.zeros(B, 2, device=self.dev), zeros, torch.arange(B, device=self.dev))
         n = _lib.launch_count() - n0
+        self.use_graph = use_graph
         self.hidden.copy_(saved[0])
         self.prev.copy_(saved[1])
         return n

@@ -138,7 +138,7 @@ class FullStep:
         # the map update is captured into a CUDA graph on its second call with the same buffers (third call overall): keep the
         # capture (tens to hundreds of ms) out of the timed region whatever `warmup` is
         extra = 0
-        while self.omb.use_graph and not self.omb._graphs and extra < 3:
+        while self.omb.use_graph and not self.omb.graphs.captured and extra < 3:
             self.step(warmup + extra, False)
             extra += 1
         torch.cuda.synchronize()

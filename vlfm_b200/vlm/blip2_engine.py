@@ -3,7 +3,7 @@
 Replaces what ``self.model({"image": img, "text_input": txt}, match_head="itc")`` does
 inside ``BLIP2ITM.cosine`` (vlfm/vlm/blip2itm.py:52) together with the preprocessing at
 :48-49.  Python here only sequences C-ABI launches over preallocated buffers; the whole
-per-batch forward is captured once in a CUDA graph and replayed.
+per-batch forward is captured in a CUDA graph on its second call and replayed (``utils/cuda_graph.py``).
 
 Numerics: fp16 GEMM/attention operands (lavis runs the ViT under fp16 autocast too),
 fp32 accumulation (registers), fp32 residual stream, fp32 LayerNorm / softmax statistics.
@@ -12,13 +12,13 @@ from __future__ import annotations
 
 import ctypes
 import math
-import os
 from typing import Dict, List, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from .. import _lib
+from ..utils.cuda_graph import GraphCache, default_use_graph
 from . import dense
 from .blip2_config import Blip2Dims
 from .preprocess import CLIP_MEAN, CLIP_STD, bicubic_tables
@@ -37,16 +37,15 @@ def partials_floats(dims: Blip2Dims, max_batch: int) -> int:
 
 
 class Blip2ITCEngine:
-    def __init__(self, dims: Blip2Dims, state_dict: Dict[str, torch.Tensor], device="cuda", max_batch: int = 1,
-                 use_graph: bool = True) -> None:
+    def __init__(self, dims: Blip2Dims, state_dict: Dict[str, torch.Tensor], device="cuda", max_batch: int = 1) -> None:
         if not torch.cuda.is_available():
             raise _lib.VlfmError("vlfm_b200 needs a CUDA device (no CPU fallback)")
         self.lib = _lib.load()
         self.d = dims
         self.dev = torch.device(device)
         self.max_batch = max_batch
-        self.use_graph = use_graph and os.environ.get("VLFM_NO_GRAPH", "") != "1"
-        self._graphs: Dict[Tuple[int, int, int], Tuple[torch.cuda.CUDAGraph, torch.Tensor]] = {}
+        self.use_graph = default_use_graph()
+        self.graphs = GraphCache()
         self._tables: Dict[Tuple[int, int], Tuple[torch.Tensor, ...]] = {}
         self._mean = (ctypes.c_float * 3)(*CLIP_MEAN)
         self._std = (ctypes.c_float * 3)(*CLIP_STD)
@@ -330,26 +329,13 @@ class Blip2ITCEngine:
         text feature last given to set_text()."""
         B, Hh, Ww, _ = images.shape
         assert B <= self.max_batch and images.dtype == torch.uint8 and images.is_contiguous()
-        key = (B, Hh, Ww)
         self.generation += 1
+
+        def run(img: torch.Tensor) -> None:
+            self._forward_impl(img, torch.empty(B, Hh, self.d.image, 3, dtype=torch.uint8, device=self.dev))
+
         with torch.cuda.device(self.dev):
-            if not self.use_graph:
-                mid = torch.empty(B, Hh, self.d.image, 3, dtype=torch.uint8, device=self.dev)
-                self._forward_impl(images, mid)
-                return self.out[:B]
-            if key not in self._graphs:
-                static_in = torch.empty_like(images)
-                mid = torch.empty(B, Hh, self.d.image, 3, dtype=torch.uint8, device=self.dev)
-                static_in.copy_(images)
-                self._forward_impl(static_in, mid)  # warm-up: function attributes, table upload
-                torch.cuda.synchronize()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    self._forward_impl(static_in, mid)
-                self._graphs[key] = (g, static_in, mid)
-            g, static_in, _ = self._graphs[key]
-            static_in.copy_(images, non_blocking=True)
-            g.replay()
+            self.graphs((B, Hh, Ww), self.use_graph, run, images)
         return self.out[:B]
 
     @torch.inference_mode()

@@ -15,6 +15,7 @@ from typing import Any, Dict, List, Optional
 import numpy as np
 import torch
 
+from ..utils.cuda_graph import GraphCache, default_use_graph
 from .detections import ObjectDetections
 from .gdino_accel import accelerate
 from .gdino_forward import GdinoForward
@@ -25,6 +26,7 @@ GROUNDING_DINO_CONFIG = "GroundingDINO/groundingdino/config/GroundingDINO_SwinT_
 GROUNDING_DINO_WEIGHTS = "data/groundingdino_swint_ogc.pth"
 CLASSES = "chair . person . dog ."  # grounding_dino.py:20
 BACKBONE_PREFIX = "model.backbone.conv_encoder.model."
+GRAPH_MAX_BATCH = 4
 
 
 class SimpleCaptionTokenizer:
@@ -123,50 +125,25 @@ class GroundingDINO:
         self._pin: Optional[torch.Tensor] = None
         self._dev: Optional[torch.Tensor] = None
         self._pin_ev: Optional[torch.cuda.Event] = None
-        self._static: Dict[Any, Dict[str, Any]] = {}
-        self._graph_ok = os.environ.get("VLFM_GDINO_GRAPH", "1") != "0"
-        self._graph_max_batch = int(os.environ.get("VLFM_GDINO_GRAPH_MAX_BATCH", "4"))
-        self.graph_error: Optional[str] = None
-
-    def _forward_static(self, st):
-        """One forward on the static buffers of ``st`` (eager or under CUDA-graph capture)."""
-        st["logits"], st["boxes"] = self.fwd.forward(st["img"], st["key_ids"])
-        st["keep"] = self.fwd.last       # a captured graph reads the cached shape / caption constants by address: keep them alive
+        self.use_graph = default_use_graph()
+        self.graphs = GraphCache(max_keys=4)
 
     @torch.inference_mode()
     def raw_outputs_device(self, images: torch.Tensor, input_ids: List[int]):
         """images [B,H,W,3] uint8 on the device -> (sigmoid logits [B,900,256], boxes [B,900,4] cxcywh).
 
-        Small batches (the per-step policy call is batch 1) replay a CUDA graph of the whole detector per
-        (batch, image size, caption): the forward is launch-bound otherwise."""
+        Batches up to GRAPH_MAX_BATCH (the per-step policy call is batch 1) replay a CUDA graph of the whole detector per
+        (batch, image size, caption) from their second call: the forward is launch-bound otherwise."""
+        ids = [int(i) for i in input_ids]
+
+        def run(img: torch.Tensor):
+            logits, boxes = self.fwd.forward(img, ids)
+            # a captured graph reads the cached shape / caption constants by address: returning them keeps them alive
+            return logits, boxes, self.fwd.last
+
         b, h, w = images.shape[:3]
-        key = (int(b), int(h), int(w), tuple(int(i) for i in input_ids))
-        st = self._static.get(key)
-        if st is None:
-            st = {"img": torch.empty_like(images), "calls": 0, "graph": None, "key_ids": list(key[3])}
-            if len(self._static) >= 4:
-                self._static.pop(next(iter(self._static)))
-            self._static[key] = st
-        st["img"].copy_(images, non_blocking=True)
-        st["calls"] += 1
-        use_graph = self._graph_ok and b <= self._graph_max_batch
-        if use_graph and st["graph"] is None and st["calls"] >= 2:       # call 1 warmed every cache up eagerly
-            try:
-                torch.cuda.synchronize()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    self._forward_static(st)
-                st["graph"] = g
-            except Exception as e:  # a sync point inside the forward: stay eager (loudly, once)
-                self._graph_ok = False
-                self.graph_error = repr(e)
-                print(f"[vlfm_b200] GroundingDINO CUDA-graph capture disabled: {e}", flush=True)
-                torch.cuda.synchronize()
-        if st["graph"] is not None:
-            st["graph"].replay()
-        else:
-            self._forward_static(st)
-        return st["logits"], st["boxes"]
+        logits, boxes, _ = self.graphs((int(b), int(h), int(w), tuple(ids)), self.use_graph and b <= GRAPH_MAX_BATCH, run, images)
+        return logits, boxes
 
     def raw_outputs(self, image: np.ndarray, input_ids: List[int]):
         """-> (sigmoid logits [900,256], boxes [900,4] cxcywh) on the device."""

@@ -16,6 +16,7 @@ import numpy as np
 import torch
 
 from .. import _lib
+from ..utils.cuda_graph import GraphCache, default_use_graph
 from .dense import conv_rows, gemm_f16, im2col
 from .yolov7_weights import Layer, fold, fold_detect
 
@@ -88,7 +89,8 @@ class YoloEngine:
         self.params = torch.zeros(8, dtype=torch.int32, device=self.dev)      # VlfmYoloParams
         self._bufs: Dict[int, dict] = {}
         self._tables: Dict[Tuple[int, int], tuple] = {}
-        self._graphs: Dict[Tuple[int, int, int], tuple] = {}
+        self.use_graph = default_use_graph()
+        self.graphs = GraphCache()
         self.set_params(0.25, 0.45, None, False)
 
     # --------------------------------------------------------------------------------------------------------- weights
@@ -385,7 +387,7 @@ class YoloEngine:
             self._tables[(H, W)] = tuple(torch.from_numpy(a).to(self.dev) for a in (yo, ys, yb, xo, xs, xa))
 
     @torch.inference_mode()
-    def run(self, images: torch.Tensor, graph: bool = True) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    def run(self, images: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
         """images [B,H,W,3] uint8 RGB (device) -> views of (boxes [B,300,4], scores [B,300], classes [B,300], counts [B]); valid
         until the next call with the same B."""
         if images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] != 3:
@@ -395,20 +397,5 @@ class YoloEngine:
         with torch.cuda.device(self.dev):
             self._prepare(H, W)
             bufs = self._buffers(B)
-            if not graph:
-                self._forward(images.contiguous(), B, H, W, bufs)
-            else:
-                key = (B, H, W)
-                if key not in self._graphs:
-                    static_in = images.contiguous().clone()
-                    self._forward(static_in, B, H, W, bufs)
-                    torch.cuda.synchronize()
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g):
-                        self._forward(static_in, B, H, W, bufs)
-                    self._graphs[key] = (g, static_in)
-                else:
-                    g, static_in = self._graphs[key]
-                    static_in.copy_(images, non_blocking=True)
-                    g.replay()
+            self.graphs((B, H, W), self.use_graph, lambda x: self._forward(x, B, H, W, bufs), images.contiguous())
         return bufs["boxes"], bufs["scores"], bufs["classes"], bufs["counts"]
