@@ -11,6 +11,8 @@
 //     feature, max over queries (blip2itm.py:52, match_head="itc").
 #include <cuda_fp16.h>
 #include <math.h>
+#include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 
@@ -249,6 +251,58 @@ __device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, co
   asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(addr));
 }
 
+// Batch-1 staging (attention_kernel<HDP, 4, true>): 64 query rows per CTA, so each head's K / V is read by ceil(Nq/64) CTAs instead
+// of ceil(Nq/32) (the ViT-g at batch 1: 80 CTAs, one wave), and nothing waits for all of it.  Shared memory: sK, sV [NKP][HDP + 8],
+// sQ [64][HDP + 8] (the merge buffer overlays them), then ATT_B1_BARS mbarriers.  Every thread issues its 16-byte cp.async copies
+// for Q, then K and V of each of the four key parts in turn, and after each piece a cp.async.mbarrier.arrive on the piece's
+// barrier (count: every thread): a barrier completes when every copy issued up to it has landed, so part 0 starts computing on
+// its keys while the other parts' are in flight.  The parts and their 64-key blocks are those of attention_kernel<HDP, 4>, so a
+// row's arithmetic, and its result, are the same.
+constexpr int ATT_B1_ROWS = 64;
+constexpr int ATT_B1_THREADS = 512;
+constexpr int ATT_B1_BARS = 5;             // Q, then K and V of each key part
+
+__host__ __device__ constexpr int attn_b1_bar_offset(int nkp, int hdp) {   // bytes; the merge of 12 warps may need more than the staging
+  return (2 * nkp + ATT_B1_ROWS) * (hdp + 8) * 2 > 12 * (hdp / 2 + 4) * 32 * 4 ? (2 * nkp + ATT_B1_ROWS) * (hdp + 8) * 2
+                                                                              : 12 * (hdp / 2 + 4) * 32 * 4;
+}
+
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const __half* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(p)));
+}
+
+template <int HDP>
+__device__ __forceinline__ void attn_b1_stage(const AttnArgs& a, uint8_t* smem, __half* sK, __half* sV, const __half* kbase,
+                                              const __half* vbase, int NKP, int qb, int tid) {
+  constexpr int KS = HDP + 8, CH = HDP / 8;
+  const uint32_t bars = smem_u32(smem + attn_b1_bar_offset(NKP, HDP));
+  if (tid == 0) {
+    for (int i = 0; i < ATT_B1_BARS; ++i) mbar_init(bars + 8 * i, ATT_B1_THREADS);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  // rows [r0, r1) of a [rows][KS] tile; src-size 0 zero-fills rows >= rlim and columns >= hd
+  auto copy_rows = [&](__half* dst, const __half* src, int ld, int r0, int r1, int rlim) {
+    for (int i = r0 * CH + tid; i < r1 * CH; i += ATT_B1_THREADS) {
+      const int r = i / CH, c = (i - r * CH) * 8;
+      const bool ok = r < rlim && c < a.hd;
+      const __half* p = ok ? src + (size_t)r * ld + c : src;
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst + r * KS + c)), "l"(p), "r"(ok ? 16 : 0) : "memory");
+    }
+  };
+  const __half* qbase = a.q + ((size_t)blockIdx.z * a.Nq + (size_t)qb * ATT_B1_ROWS) * a.ldq + (size_t)blockIdx.y * a.hd;
+  copy_rows(sV + NKP * KS, qbase, a.ldq, 0, ATT_B1_ROWS, min(ATT_B1_ROWS, a.Nq - qb * ATT_B1_ROWS));
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bars) : "memory");
+  const int tiles = NKP >> 4, tbase = tiles / 4, trem = tiles % 4;
+  for (int p = 0; p < 4; ++p) {
+    const int k0 = 16 * (p * tbase + min(p, trem)), k1 = k0 + 16 * (tbase + (p < trem ? 1 : 0));
+    copy_rows(sK, kbase, a.ldk, k0, k1, a.Nk);
+    copy_rows(sV, vbase, a.ldv, k0, k1, a.Nk);
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bars + 8 * (1 + p)) : "memory");
+  }
+}
+
 // grid (ceil(Nq/32), heads, B), 4 warps.  K and V of one (batch, head) are staged row-major
 // [key][hd] in padded (conflict-free) shared memory with 16-byte copies.  Warp w owns query rows
 // 16*(w&1).. and the key half (w>>1); the two halves are merged flash-style through shared memory.
@@ -257,10 +311,12 @@ __device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, co
 // KH = 2: 32 query rows per CTA, each row group's keys split over two warps (small batches: more CTAs,
 // shorter critical path).  KH = 1: 64 query rows per CTA, every warp sees all keys (large batches: the K/V
 // staging is amortised over twice the queries, no merge).
-template <int HDP, int KH>
-__global__ void __launch_bounds__(32 * (KH == 4 ? 8 : ATT_WARPS))
+template <int HDP, int KH, bool B1 = false>
+__global__ void __launch_bounds__(32 * (B1 ? 16 : (KH == 4 ? 8 : ATT_WARPS)))
 attention_kernel(AttnArgs a) {
-  constexpr int NW = KH == 4 ? 8 : ATT_WARPS;   // KH = 4: eight warps = 2 row groups x 4 key quarters (batch 1: shortest critical path)
+  static_assert(!B1 || KH == 4, "the batch-1 variant splits the keys in four");
+  // KH = 4: eight warps = 2 row groups x 4 key quarters (small batches: shortest critical path); B1: sixteen = 4 x 4
+  constexpr int NW = B1 ? 16 : (KH == 4 ? 8 : ATT_WARPS);
   constexpr int RG = NW / KH;            // row groups of 16 queries
   constexpr int ATT_QBLK = 16 * RG;
   constexpr int KS = HDP + 8;            // row stride (halves) of sK / sV
@@ -275,9 +331,12 @@ attention_kernel(AttnArgs a) {
   const __half* kbase = a.k + (size_t)b * a.Nk * a.ldk + (size_t)h * a.hd;
   const __half* vbase = a.v + (size_t)b * a.Nk * a.ldv + (size_t)h * a.hd;
 
+  constexpr int CH = HDP / 8;
+  if constexpr (B1) {
+    attn_b1_stage<HDP>(a, att_smem, sK, sV, kbase, vbase, NKP, qb, tid);
+  } else {
   // ---- stage K and V with cp.async (16-byte LDGSTS, all copies in flight at once; src-size 0 zero-fills the
   // padding rows >= Nk and columns >= hd)
-  constexpr int CH = HDP / 8;
   for (int i = tid; i < NKP * CH; i += 32 * NW) {
     const int key = i / CH, c = (i - key * CH) * 8;
     const bool ok = key < a.Nk && c < a.hd;
@@ -289,13 +348,17 @@ attention_kernel(AttnArgs a) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(vd), "l"(vsrc), "r"(nbytes) : "memory");
   }
   asm volatile("cp.async.commit_group;" ::: "memory");
+  }
 
   // ---- Q fragments: rows 16*(warp&1) + {g, g+8} of this CTA's 32-row block
   const int row0 = qb * ATT_QBLK + (warp % RG) * 16;
   const int r_lo = row0 + g, r_hi = row0 + g + 8;
+  uint32_t qf[HDP / 16][4];
+  if constexpr (B1) {   // Q fragments: read from sQ in each key block (fewer registers live across P.V: 16 warps of 128)
+    mbar_wait(smem_u32(att_smem + attn_b1_bar_offset(NKP, HDP)), 0);
+  } else {
   const __half* qlo = a.q + ((size_t)b * a.Nq + r_lo) * a.ldq + (size_t)h * a.hd;
   const __half* qhi = a.q + ((size_t)b * a.Nq + r_hi) * a.ldq + (size_t)h * a.hd;
-  uint32_t qf[HDP / 16][4];
 #pragma unroll
   for (int kk = 0; kk < HDP / 16; ++kk) {
     const int c0 = kk * 16 + 2 * t, c1 = c0 + 8;
@@ -306,6 +369,7 @@ attention_kernel(AttnArgs a) {
   }
   asm volatile("cp.async.wait_group 0;" ::: "memory");
   __syncthreads();
+  }
 
   float o[HDP / 8][4];
 #pragma unroll
@@ -315,8 +379,14 @@ attention_kernel(AttnArgs a) {
   // key range of this warp: the 16-key tiles are dealt to the KH parts, the first parts take the remainder
   const int part = warp / RG, tiles = NKP >> 4, tbase = tiles / KH, trem = tiles % KH;
   const int k_begin = 16 * (part * tbase + min(part, trem)), k_end = k_begin + 16 * (tbase + (part < trem ? 1 : 0));
+  if constexpr (B1) mbar_wait(smem_u32(att_smem + attn_b1_bar_offset(NKP, HDP)) + 8 * (1 + part), 0);   // K and V of this part
   for (int kb = k_begin; kb < k_end; kb += 64) {
     const int ntiles = min(8, (k_end - kb) >> 3);   // warp-uniform, even
+    if constexpr (B1) {   // ldmatrix.x4: lanes 0-15 address rows +0..15 at column 16 kk, lanes 16-31 at 16 kk + 8
+      const __half* qr = sV + NKP * KS + ((warp % RG) * 16 + (lane & 15)) * KS + (lane >> 4) * 8;
+#pragma unroll
+      for (int kk = 0; kk < HDP / 16; ++kk) ldmatrix_x4(qf[kk], qr + kk * 16);
+    }
     float s[8][4];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -743,6 +813,32 @@ extern "C" int vlfm_attention_f16(const void* d_q, const void* d_k, const void* 
   AttnArgs a{(const __half*)d_q, (const __half*)d_k, (const __half*)d_v, (__half*)d_o, ldq, ldk, ldv, ldo, Nq, Nk, hd, heads,
              scale * 1.4426950408889634f};
   cudaStream_t st = (cudaStream_t)stream;
+  // VLFM_ATT_IMPL: unset = by shape; "legacy" = never the batch-1 kernel; "b1" = the batch-1 kernel for every shape (tests)
+  const char* impl = getenv("VLFM_ATT_IMPL");
+  const bool force_legacy = impl && !strcmp(impl, "legacy"), force_b1 = impl && !strcmp(impl, "b1");
+  if (impl && impl[0] && !force_legacy && !force_b1) { set_error("vlfm_attention_f16: VLFM_ATT_IMPL=%s (legacy or b1)", impl); return VLFM_E_INVALID; }
+  const size_t nkp = ((size_t)Nk + 15) & ~(size_t)15;
+  const int hdp = hd <= 64 ? 64 : 96;
+  // the batch-1 kernel when its 64-row blocks fit one wave of one CTA per SM and the keys fill at least one 64-key chunk (the
+  // ViT-g at batch 1); the short attentions of MobileSAM and every larger batch keep the variants below
+  const long items64 = (long)B * heads * ((Nq + ATT_B1_ROWS - 1) / ATT_B1_ROWS);
+  if (force_b1 || (!force_legacy && items64 <= 132 && Nk >= 64)) {
+    static bool cfg_b1 = false;
+    if (!cfg_b1) {
+      const int mx = attn_b1_bar_offset(ATT_NKMAX, 96) + 8 * ATT_B1_BARS;
+      int rc = check_cuda(cudaFuncSetAttribute(attention_kernel<64, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx), "attr(attention b1)");
+      if (!rc) rc = check_cuda(cudaFuncSetAttribute(attention_kernel<96, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx), "attr(attention b1)");
+      if (rc) return rc;
+      cfg_b1 = true;
+    }
+    const size_t sm = attn_b1_bar_offset((int)nkp, hdp) + 8 * ATT_B1_BARS;
+    const dim3 grid((Nq + ATT_B1_ROWS - 1) / ATT_B1_ROWS, heads, B);
+    cudaError_t e = hdp == 64 ? launch_pdl(attention_kernel<64, 4, true>, grid, dim3(ATT_B1_THREADS), sm, st, a)
+                              : launch_pdl(attention_kernel<96, 4, true>, grid, dim3(ATT_B1_THREADS), sm, st, a);
+    { int rc = check_cuda(e, "attention_kernel (batch 1)"); if (rc) return rc; }
+    count_launch();
+    return VLFM_OK;
+  }
   // few (batch, head, block) work items -> 32-row blocks with split keys (4-way when they fit one wave of 8-warp CTAs,
   // else 2-way); many -> 64-row blocks
   const long items = (long)B * heads * ((Nq + 31) / 32);
@@ -752,7 +848,6 @@ extern "C" int vlfm_attention_f16(const void* d_q, const void* d_k, const void* 
   const bool quad = !big && kh4 && items <= 264 && Nk >= 64;
   const int qblk = big ? 64 : 32;
   dim3 grid((Nq + qblk - 1) / qblk, heads, B);
-  const size_t nkp = ((size_t)Nk + 15) & ~(size_t)15;
   static bool cfg = false;
   if (!cfg) {
     int rc = check_cuda(cudaFuncSetAttribute(attention_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * ATT_NKMAX * (64 + 8) * 2), "attr(attention)");
@@ -764,7 +859,6 @@ extern "C" int vlfm_attention_f16(const void* d_q, const void* d_k, const void* 
     if (rc) return rc;
     cfg = true;
   }
-  const int hdp = hd <= 64 ? 64 : 96;
   size_t sm = 2 * nkp * (hdp + 8) * 2;
   if (sm < 6 * 52 * 32 * 4) sm = 6 * 52 * 32 * 4;   // merge buffer of the split-key variants
   cudaError_t e;
